@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- frames/s of the ProPainter inference hot path on B200 (contract in the task statement).
+"""bench.py -- frames/s of the ProPainter inference hot path on H100.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload c2|c1|c3|c4|c5] [--no-cpu-baseline]
-                  [--no-gpu-reference] [--no-strong] [--shard]
+                  [--no-gpu-reference] [--no-strong] [--shard] [--dump-outputs DIR]
 
 A "step" is one full pass of stages 1-4 (RAFT flow -> flow completion -> image propagation ->
 sliding-window generator + compositing) over one synthetic clip.  N=1 workload = BASELINE.json
@@ -17,6 +17,7 @@ propainter_b200/dist.py (point-to-point halo exchange over NCCL), at every N inc
 of the long-clip configuration can be read off the per-N lines.
 --impl reference: the oracle (CPU restatement of the reference's PyTorch path) on the host cores
 over a bounded sample of the same workload.
+--dump-outputs DIR: the composited video of the last timed step, as .npy (dump_outputs); inputs and weights are seeded.
 """
 import argparse
 import json
@@ -46,12 +47,29 @@ STRONG_WORKLOAD = "c4"     # the long clip of BASELINE.json configs[3] that `str
 CPU_SAMPLE_FRAMES = 6      # bounded sample of the same workload for the CPU arm (full clip ~ 10 min of CPU)
 
 
+DUMP_LIMIT_BYTES = 64_000_000
+
+
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1590.0, "fallback (B200_PROFILING.md)"
+    """H100 SXM data-sheet figures: 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 (700 W card; a lower power limit lowers what
+    is reachable, see the `clocks` block of the line)."""
+    return 3350.0, 989.0, "H100 SXM data sheet (dense)"
+
+
+def dump_outputs(out_dir, arrays):
+    """<out_dir>/<name>.npy in float32; past the size budget a fixed seeded sample (<name>_sample.npy) + its flat indices"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    budget = DUMP_LIMIT_BYTES // len(arrays)
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.float32)
+        if a.nbytes <= budget:
+            np.save(os.path.join(out_dir, name + ".npy"), a)
+            continue
+        n = (budget - 4096) // 12                                # float32 value + float64 index per element; 4 KB for the .npy headers
+        idx = np.sort(np.random.default_rng(0).choice(a.size, size=n, replace=False))
+        np.save(os.path.join(out_dir, name + "_sample.npy"), a.reshape(-1)[idx])
+        np.save(os.path.join(out_dir, name + "_sample_index.npy"), idx.astype(np.float64))
 
 
 class ClockSampler:
@@ -258,17 +276,12 @@ def _time_kernel(torch, fn, reps=10):
 def roofline_probe(torch, pipe, wl):
     """Live roofline of our dominant kernels at the workload's shapes (DESIGN.md §4/§5).
 
-    Primary entry = the tensor-core kernel the north star names (sparse window attention, tcgen05/TMEM); the
-    `others` list carries the HBM-bound RAFT lookup and the deformable alignment.  ncu DRAM traffic figures
-    (`traffic`, bytes per launch) come from the committed capture profiles/r2_ncu_kernels.csv (dram__bytes_read.sum +
-    dram__bytes_write.sum of one `ncu --set full` pass over profiles/ncu_targets.py at these shapes; the lookup figure is the
-    22-pair capture scaled to the batch; they cannot be measured outside a profiler and are only attached at the C2 shapes)."""
+    Primary entry = the tensor-core kernel the north star names (sparse window attention, wgmma); the
+    `others` list carries the HBM-bound RAFT lookup and the deformable alignment."""
     from propainter_b200 import ops
     from propainter_b200.window_index import padded_grid, token_grid, window_key_table
-    c2 = (wl["H"], wl["W"]) == (240, 432)
-    ncu = (lambda mb: int(mb * 1e6)) if c2 else (lambda mb: None)
     hbm, bf16, src = peaks()
-    tf32_peak = bf16 / 2.0                                          # tcgen05 kind::tf32 runs at half the bf16 rate
+    tf32_peak = bf16 / 2.0                                          # TF32 tensor-core rate = half the bf16 rate
     dev = pipe.device
     # ---- sparse window attention: one transformer layer of a full generator window (t = 18 frames)
     t, C = 18, 512
@@ -287,7 +300,7 @@ def roofline_probe(torch, pipe, wl):
     ms = _time_kernel(torch, lambda: ops.sparse_window_attn(qkv, pool, ktab, flags, t, H2 * W2, 0, 2))
     ach = flops / (ms * 1e-3) / 1e12
     primary = {"kernel": "k_sparse_attn_umma (+ unmasked-window kernel)", "bound": "tensor", "achieved": ach, "peak": tf32_peak,
-               "unit": "TFLOP/s", "frac": ach / tf32_peak, "traffic": ncu(29.62 + 0.21), "peak_source": src + " bf16_tflops / 2 (TF32)",
+               "unit": "TFLOP/s", "frac": ach / tf32_peak, "peak_source": src + " bf16_tflops / 2 (TF32)",
                "launch_ms": ms, "algorithmic_flops": flops, "masked_windows": f"{nmask} of {nwin}"}
     # ---- RAFT correlation lookup, one refinement step of the whole clip
     h, w = wl["H"] // 8, wl["W"] // 8
@@ -303,7 +316,7 @@ def roofline_probe(torch, pipe, wl):
     npx = h * w
     alg = B * (npx * 4 * 100 * 4 + npx * 324 * 4 + npx * 8)        # unique 10x10 patches at 4 levels + 324-ch output + coords
     ach_l = alg / (ms_l * 1e-3) / 1e9
-    # ---- deformable alignment, one generator propagation step: sampling kernel + tcgen05 GEMM over the sampled columns
+    # ---- deformable alignment, one generator propagation step: sampling kernel + wgmma GEMM over the sampled columns
     Hh, Ww = wl["H"] // 4, wl["W"] // 4
     x, o = torch.randn(1, Hh, Ww, 128, device=dev), torch.randn(1, Hh, Ww, 432, device=dev)
     fl = torch.randn(1, Hh, Ww, 2, device=dev)
@@ -313,7 +326,7 @@ def roofline_probe(torch, pipe, wl):
     ms_g = _time_kernel(torch, lambda: ops.deform_gather(x, o, fl, 3.0, cols))
     ms_m = _time_kernel(torch, lambda: ops.conv_umma([cols], wd, 1, 1, 128, bias=bvec, out=dout))
     fl_d = Hh * Ww * 9 * 128 * 128 * 2
-    # ---- the tcgen05 conv kernel on one 3x3 128->128 conv of a generator propagation step (bias + LeakyReLU + residual fused)
+    # ---- the wgmma conv kernel on one 3x3 128->128 conv of a generator propagation step (bias + LeakyReLU + residual fused)
     xc = torch.randn(1, Hh, Ww, 128, device=dev)
     wc = ops.pack_conv_weight(torch.randn(128, 128, 3, 3, device=dev) * 0.03)
     rc, oc = torch.randn(1, Hh, Ww, 128, device=dev), torch.empty(1, Hh, Ww, 128, device=dev)
@@ -321,14 +334,14 @@ def roofline_probe(torch, pipe, wl):
     fl_c = Hh * Ww * 9 * 128 * 128 * 2
     primary["others"] = [
         {"key": "corr_lookup", "kernel": "k_corr_lookup_tma", "bound": "hbm", "achieved": ach_l, "peak": hbm, "unit": "GB/s", "frac": ach_l / hbm,
-         "traffic": ncu((107.34 + 18.49) * B / 22.0), "launch_ms": ms_l, "algorithmic_bytes": alg},
+         "launch_ms": ms_l, "algorithmic_bytes": alg},
         {"key": "deform", "kernel": "k_deform_gather + k_conv_umma (1x1 over the sampled columns)", "bound": "tensor",
          "achieved": fl_d / ((ms_g + ms_m) * 1e-3) / 1e12, "peak": tf32_peak, "unit": "TFLOP/s",
-         "frac": fl_d / ((ms_g + ms_m) * 1e-3) / 1e12 / tf32_peak, "traffic": ncu(14.60 + 0.03 + 30.52 + 0.02), "launch_ms": ms_g + ms_m, "gather_ms": ms_g, "gemm_ms": ms_m,
+         "frac": fl_d / ((ms_g + ms_m) * 1e-3) / 1e12 / tf32_peak, "launch_ms": ms_g + ms_m, "gather_ms": ms_g, "gemm_ms": ms_m,
          "algorithmic_flops": fl_d, "note": "two launches; the gather is L2-bandwidth bound (119 MB of corner reads per step)"},
         {"key": "conv", "kernel": "k_conv_umma 3x3 128->128 on the 60x108 map", "bound": "tensor", "achieved": fl_c / (ms_c * 1e-3) / 1e12,
-         "peak": tf32_peak, "unit": "TFLOP/s", "frac": fl_c / (ms_c * 1e-3) / 1e12 / tf32_peak, "traffic": ncu(10.61), "launch_ms": ms_c,
-         "algorithmic_flops": fl_c, "note": "single launch incl. launch latency; 112 CTAs on 148 SMs; tf32 operands from shared memory"}]
+         "peak": tf32_peak, "unit": "TFLOP/s", "frac": fl_c / (ms_c * 1e-3) / 1e12 / tf32_peak, "launch_ms": ms_c,
+         "algorithmic_flops": fl_c, "note": "single launch incl. launch latency; tf32 operands from shared memory"}]
     return primary
 
 
@@ -407,16 +420,19 @@ def run_ours(args, wl):
     if args.windows_in_flight:
         cfg.windows_in_flight = args.windows_in_flight
     u8_dev, fm_dev, md_dev = u8_host.to(dev), fm_host.to(dev), md_host.to(dev)
-    flush = torch.empty(64 * 1024 * 1024, device=dev)          # 256 MiB > 126 MB L2
+    flush = torch.empty(64 * 1024 * 1024, device=dev)          # 256 MiB > 50 MB L2
 
     runner = pipe
     if shard:                                                  # one clip time-sharded over the ranks (propainter_b200/dist.py)
         from propainter_b200.dist import ShardedProPainter
         runner = ShardedProPainter(pipe)
 
+    last = {}                                                  # output of the latest resident step (--dump-outputs)
+
     def step_resident():
         r = runner(u8_dev, fm_dev, md_dev, cfg)
-        return r[0] if shard else r
+        last["comp"] = r[0] if shard else r
+        return last["comp"]
 
     def step_e2e():
         r = runner(u8_host, fm_host, md_host, cfg)             # H2D inside
@@ -472,7 +488,7 @@ def run_ours(args, wl):
                 if e2e:
                     outs[k].copy_(pipes[k](u8_host, fm_host, md_host, cfg), non_blocking=True)
                 else:
-                    pipes[k](u8_dev, fm_dev, md_dev, cfg)
+                    last["comp"] = pipes[k](u8_dev, fm_dev, md_dev, cfg)
             main = torch.cuda.current_stream()
             for st in streams:
                 st.wait_stream(main)
@@ -508,10 +524,14 @@ def run_ours(args, wl):
         ms_one, _, _ = timed(step_resident, min(args.steps, 3), args.warmup)          # latency of one clip alone, for the record
         single = {"ms_per_clip": ms_one / min(args.steps, 3), "frames_per_s": wl["T"] * min(args.steps, 3) / (ms_one * 1e-3)}
         ms_total, launches, clocks = timed_pipelined(False, args.steps, args.warmup)
+        comp_last = last["comp"].cpu().numpy()
         ms_e2e, _, _ = timed_pipelined(True, args.steps, 1)
     else:
         ms_total, launches, clocks = timed(step_resident, args.steps, args.warmup, True)
+        comp_last = last["comp"].cpu().numpy()
         ms_e2e, _, _ = timed(step_e2e, args.steps, 1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"comp": comp_last})
     strong = None
     frames_total = wl["T"] * (1 if shard else world) * args.steps
     if rank == 0:
@@ -551,9 +571,16 @@ def run_ours(args, wl):
             except Exception as exc:
                 line["gpu_reference"] = {"error": repr(exc)}
     if not args.no_strong and not shard and args.workload == "c2":
-        # last GPU block: its engine (own graph caches) is dropped afterwards.  Every rank takes part.
+        # last GPU block: its engine (own graph caches) is dropped afterwards.  Every rank takes part.  The C2 engine's
+        # captured graphs are released first: their private pools would otherwise stay pinned next to the 720p clip's.
         try:
             import gc
+            for v in vars(pipe).values():
+                if isinstance(v, torch.nn.Module):
+                    for m in v.modules():
+                        if hasattr(m, "graphs"):
+                            m.graphs.clear()
+            gc.collect()
             torch.cuda.empty_cache()
             torch.cuda.reset_peak_memory_stats(dev)
             spipe = ProPainterPipeline(device=dev)
@@ -590,6 +617,8 @@ def main():
     ap.add_argument("--clips-in-flight", type=int, default=1,
                     help="engine replicas per GPU working on consecutive clips concurrently (each step is still one full clip)")
     ap.add_argument("--shard", action="store_true", help="N>1: cooperate on ONE clip (strong scaling) instead of one clip per rank")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the composited video of the last timed step to DIR as .npy (float32, <= 64 MB)")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-/* propainter_b200 -- C ABI of the sm_100a hot-path kernels (libpropainter_b200.so).
+/* propainter_b200 -- C ABI of the sm_90a hot-path kernels (libpropainter_b200.so).
  *
  * The reference (sczhou/ProPainter) has no native code and no FFI: every op below replaces a
  * *library call site* in the reference's Python (torch / torchvision), cited per entry point.
@@ -67,7 +67,7 @@ size_t pp_deform_align_workspace_bytes(int H, int W);   /* decoded tap records +
 int pp_deform_align(const float* x, int ld_x, const float* o, int ld_o, const float* o_bias, const float* flow, float max_res,
                     const float* w_packed, const float* bias, float* out, int ld_out, int H, int W, int Cin, int Cout,
                     void* workspace, size_t ws_bytes, cudaStream_t stream);
-/* ---- tcgen05 convolution (conv_umma.cu) -------------------------------------------------------- */
+/* ---- wgmma convolution (conv_umma.cu) ---------------------------------------------------------- */
 /* Stride-1 "same" KHxKW convolution + the epilogue that follows it in the reference, as one kernel:
  *   out = post_relu?( act( conv(cat(seg...), W) + bias + pre ) + res )        [optionally rounded to TF32 on store]
  * Replaces F.conv2d / nn.Conv2d (cuDNN) + bias + nn.LeakyReLU/ReLU + residual add + torch.cat of the recurrent
@@ -135,7 +135,7 @@ typedef struct PPAttnParams {
 } PPAttnParams;
 /* SparseWindowAttention.forward model/modules/sparse_transformer.py:177-275 (between q/k/v and proj). */
 int pp_sparse_window_attn(const PPAttnParams* prm, int n_windows, cudaStream_t stream);
-/* same contract; masked windows on the warp-level mma.sync kernel (baseline of the tcgen05/TMEM kernel) */
+/* same contract; masked windows on the warp-level mma.sync kernel (baseline of the wgmma kernel) */
 int pp_sparse_window_attn_mma(const PPAttnParams* prm, int n_windows, cudaStream_t stream);
 
 /* FusionFeedForward.forward model/modules/sparse_transformer.py:81-100: fold -> /normalizer -> unfold -> GELU.

@@ -1,8 +1,5 @@
-"""Checks + times the tcgen05 attention kernel of whichever library build PROPAINTER_B200_LIB points at against the
-mma.sync kernel (same inputs as ncu_targets.py).  Used to validate the UA_V_MN=1 build (row-major V as an MN-major
-SWIZZLE_128B_BASE32B operand):
-  nvcc ... -DUA_V_MN=1 -o propainter_b200/libpropainter_b200_vmn.so <sources>
-  PROPAINTER_B200_LIB=$PWD/propainter_b200/libpropainter_b200_vmn.so python profiles/attn_vmn_check.py"""
+"""Checks + times the wgmma attention kernel of whichever library build PROPAINTER_B200_LIB points at against the
+mma.sync kernel (same inputs as ncu_targets.py):  python profiles/attn_vmn_check.py"""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""Hardware check + timing of the tcgen05 conv kernel (pp_conv2d_umma) and the deformable gather (pp_deform_gather).
+"""Hardware check + timing of the wgmma conv kernel (pp_conv2d_umma) and the deformable gather (pp_deform_gather).
 
     python profiles/conv_check.py [group]        group in {basic, shapes, deform, step}; default all, one subprocess each
 

@@ -49,7 +49,7 @@ for tag, (H, W, Cin, use_flow, mr) in {"gen": (60, 108, 128, True, 3.0), "rfc": 
     out = torch.empty(H, W, 128, device=dev)
     run(f"deform_align_{tag}", lambda: ops.deform_align(x, o, fl, mr, wp, b, out))
 
-# ---- tcgen05 conv kernel + deformable gather + flow warp at the two propagation-scan shapes
+# ---- wgmma conv kernel + deformable gather + flow warp at the two propagation-scan shapes
 for tag, (H, W) in {"gen": (60, 108), "rfc": (30, 54)}.items():
     xc = torch.randn(1, H, W, 128, device=dev)
     wpk = ops.pack_conv_weight(torch.randn(128, 128, 3, 3, device=dev) * 0.03)

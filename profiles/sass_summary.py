@@ -1,8 +1,8 @@
-"""SASS evidence per kernel: counts of the Blackwell-native / legacy mnemonics in the shipped library.
+"""SASS evidence per kernel: counts of the Hopper tensor-core / TMA / legacy mnemonics in the shipped library.
 
-    python profiles/sass_summary.py > profiles/sass_summary.txt      (needs cuobjdump + c++filt; no GPU)
+    python profiles/sass_summary.py      (needs cuobjdump + c++filt; no GPU)
 
-UTC*MMA = tcgen05.mma, UTCBAR = tcgen05.commit, LDTM / STTM = tcgen05.ld / st, UTMALDG = TMA tensor load, HMMA = legacy
+HGMMA = wgmma, WARPGROUP = wgmma fence / arrive, UTMALDG = TMA tensor load, HMMA = legacy
 mma.sync, LDGSTS = cp.async, SYNCS = mbarrier ops, ELECT = elect.sync (single-lane issue from a converged warp)."""
 import collections
 import os
@@ -13,7 +13,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "propainter_b200", "libpropainter_b200.so")
 txt = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True).stdout
-cols = ["UTCHMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "HMMA", "LDGSTS", "SYNCS", "ELECT"]
+cols = ["HGMMA", "WARPGROUP", "UTMALDG", "HMMA", "LDGSTS", "SYNCS", "ELECT"]
 rows = []
 for f in re.split(r"\n\s*Function : ", txt)[1:]:
     cnt = collections.Counter(m.group(1) for m in re.finditer(r"\b(" + "|".join(cols) + r")\b", f))

@@ -1,4 +1,4 @@
-"""RAFT optical flow (basic model) on the B200 hot path.
+"""RAFT optical flow (basic model) on the H100 hot path.
 
 Drop-in for the reference's ``RAFT`` (RAFT/raft.py:24-146): same constructor argument, same
 ``forward(image1, image2, iters, flow_init, test_mode)`` result in test mode, same state_dict.

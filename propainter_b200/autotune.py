@@ -22,9 +22,11 @@ def pick(key, variants, *args, reps=5, graph_timed=False):
     """graph_timed: time every candidate as a captured CUDA graph (device time of the launch sequence, the way the stage
     will actually run) instead of eagerly -- for plans made of many small kernels an eager timing measures the host's
     launch rate, not the GPU."""
+    if not args[0].is_cuda:                                 # choices are measured on the GPU: CPU inputs always run candidate 0
+        return variants[0](*args)
     i = _choice.get(key)
     if i is None:
-        if not config.AUTOTUNE or not args[0].is_cuda or torch.cuda.is_current_stream_capturing():
+        if not config.AUTOTUNE or torch.cuda.is_current_stream_capturing():
             return variants[0](*args)
         best, i = None, 0
         for j, fn in enumerate(variants):

@@ -9,7 +9,7 @@ CUDNN_BENCHMARK let cuDNN autotune conv algorithms during graph warm-up.
 CUDA_GRAPHS     replay each stage as a captured CUDA graph per shape signature (propainter_b200/graphs.py).
 FUSED_EPILOGUE  conv bias + activation through pp_bias_act (one pass) instead of cuDNN's bias add_ + ATen activation.
 UMMA_CONV       the convolutions of the two recurrent propagation scans (offset nets, backbones, deformable-conv GEMM) run on
-                the tcgen05 implicit-GEMM kernel pp_conv2d_umma (TF32 products, fused bias / activation / residual / concat
+                the wgmma implicit-GEMM kernel pp_conv2d_umma (TF32 products, fused bias / activation / residual / concat
                 epilogue) instead of cuDNN + pp_bias_act + the mma.sync deform kernel.  True / False force one plan;
                 "hybrid" keeps the library convs and replaces only the deformable conv by pp_deform_gather + a 1x1
                 pp_conv2d_umma GEMM; "hoisted" additionally convolves the step-independent input channels of
@@ -33,7 +33,7 @@ CUDNN_BENCHMARK = True
 CUDA_GRAPHS = True
 FUSED_EPILOGUE = True
 AUTOTUNE = True
-GRAPH_MAX_INPUT_BYTES = 512 << 20
+GRAPH_MAX_INPUT_BYTES = 256 << 20      # C2 calls (<= ~170 MB) are graphed; 720p calls run eagerly (80 GB)
 SCAN_PRIORITY = os.environ.get("PP_SCAN_PRIORITY", "1") != "0"
 _u = os.environ.get("PP_UMMA_CONV", "auto")
 UMMA_CONV = _u if _u in ("auto", "hybrid", "hoisted") else (_u != "0")

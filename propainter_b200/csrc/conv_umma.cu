@@ -1,4 +1,4 @@
-// Implicit-GEMM stride-1 "same" convolution on the 5th-generation tensor cores (tcgen05 / TMEM / TMA), sm_100a.
+// Implicit-GEMM stride-1 "same" convolution on the warpgroup tensor-core instructions (wgmma, TMA, mbarrier), sm_90a.
 //
 // Replaces the cuDNN convolutions of the two recurrent propagation scans -- the offset nets and backbones of
 // BidirectionalPropagation (model/propainter.py:42-50,86-96,121-175; model/recurrent_flow_completion.py:17-29,60-116) --
@@ -9,18 +9,19 @@
 //
 //   out[p][n] = post( act( sum_{seg,c,dy,dx} W[n][seg,c,dy,dx] * x_seg[p + (dy,dx)][c]  + bias[n] + pre[p][n] ) + res[p][n] )
 //
-// One CTA = one 128-pixel tile (BH x BW pixels of one map, BH*BW = 128 = UMMA M) x BN output channels.
+// One CTA = one M-pixel tile (BH x BW pixels of one map, M = BH*BW = 128 or 64) x BN output channels.
 //   * A operand: no im2col.  For every 32-channel block TMA lands KW shifted copies of the (BH+KH-1) x BW halo box
 //     (4-D tiled tensor map, SWIZZLE_128B; out-of-range rows/columns/channels are zero-filled by the TMA unit = the conv's
 //     zero padding and the channel padding to a multiple of 32).  A box is [(BH+KH-1)*BW rows][128 B] = exactly the K-major
-//     SWIZZLE_128B layout tcgen05 wants, and tap row dy is the same box read from row dy*BW on: a shared-memory descriptor
+//     SWIZZLE_128B layout wgmma wants, and tap row dy is the same box read from row dy*BW on: a shared-memory descriptor
 //     whose start address moves by dy*BW*128 B (a multiple of the 1 KB swizzle atom), so one copy feeds KH taps.
 //   * B operand: packed weights [Cout][K], K index = ((blk*KH + dy)*KW + dx)*32 + c, loaded as [BN x 32] K-major boxes.
-//   * D: 128 lanes x BN fp32 columns in TMEM; kind::tf32 (weights are pre-rounded to TF32 at pack time; activations
-//     written by this kernel are optionally rounded on store so the next conv's operands are round-to-nearest TF32 too).
-// Warp roles: warps 0-3 epilogue (thread <-> TMEM lane <-> pixel), warp 4 TMA producer, warp 5 TMEM allocator + MMA issuer.
-// Two rings: A (one slot per 32-channel block) and B (one slot per (block, dy) = KW taps).  mbarrier full/empty pairs,
-// tcgen05.commit releases slots.  Descriptor / instruction encodings: pp_umma.cuh (validated on B200, round 1).
+//   * D: fp32 registers of the consumer warpgroups (warpgroup w: pixels 64w .. 64w+63 of the tile, m64nBNk8 per k-step);
+//     TF32 products (weights are pre-rounded to TF32 at pack time; activations written by this kernel are optionally rounded
+//     on store so the next conv's operands are round-to-nearest TF32 too).
+// Warp roles: warps 0-7 two consumer warpgroups (wgmma issue + epilogue; the second idles on 64-pixel tiles), warp 8 TMA
+// producer.  Two rings: A (one slot per 32-channel block) and B (one slot per (block, dy) = KW taps), mbarrier full/empty
+// pairs; a consumer releases a slot once the wgmma group that read it has retired.  Descriptor encodings: pp_umma.cuh.
 #include <cuda.h>
 #include <stdlib.h>
 #include "pp_elem.cuh"
@@ -28,7 +29,7 @@
 #include "pp_umma.cuh"
 #include "../../include/propainter_b200.h"
 
-#define CV_THREADS 192
+#define CV_THREADS 288
 #define CV_MAX_A_SLOTS 6
 #define CV_MAX_B_SLOTS 8
 #define CV_SMEM_BUDGET (216 * 1024)
@@ -39,32 +40,18 @@ struct alignas(64) CVParams {
   int seg_blocks[PP_CONV_MAX_SEG];   // pipeline blocks per segment (kgroup: groups of KW 32-channel blocks)
   int seg_kblocks[PP_CONV_MAX_SEG];  // real 32-channel blocks per segment (= K extent of the segment / 32 per tap)
   int nseg, nblk, kreal;      // nblk pipeline blocks; kreal real 32-channel blocks
-  int n, H, W, KH, KW, BH, BW, BN, M;    // M = BH*BW = 128 or 64 (UMMA M)
+  int n, H, W, KH, KW, BH, BW, BN, M;    // M = BH*BW = 128 or 64 (pixels per CTA, one m64 warpgroup tile per 64)
   int kgroup;                 // 1x1 convs: the `KW` loop walks `KW` consecutive 32-channel blocks (one pipeline stage = KW blocks)
   int tiles_x, tiles_y;
   int na, nb;                 // ring depths
-  int ring_bytes;             // A ring + B ring, at least what the epilogue staging tiles need (4 warps x BN/32 x 4.5 KB)
+  int ring_bytes;             // A ring + B ring
   int a_copy_bytes;           // (BH+KH-1)*BW*128
   int Cout;
   const float* bias; const float* pre; const float* res; float* out;
   int ld_pre, ld_res, ld_out;
   int act, post_relu, round_tf32;
   float slope;
-#ifdef CV_PROFILE
-  long long* prof;
-#endif
 };
-
-#ifdef CV_PROFILE
-// profiling variant (profiles/build_variant.py prof -DCV_PROFILE=1): per-CTA cycle attribution written to a caller buffer
-static long long* g_cv_prof = nullptr;
-extern "C" void pp_conv_profile_buffer(long long* p) { g_cv_prof = p; }
-#define CV_CLK() clock64()
-#define CV_PROF(i, v) do { if (p.prof) p.prof[(long)(blockIdx.y * gridDim.x + blockIdx.x) * 16 + (i)] = (v); } while (0)
-#else
-#define CV_CLK() 0LL
-#define CV_PROF(i, v) do { } while (0)
-#endif
 
 __device__ __forceinline__ void cv_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -77,71 +64,51 @@ __device__ __forceinline__ void cv_tma2(uint32_t dst, const CUtensorMap* tm, int
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                ::"r"(dst), "l"(tm), "r"(k), "r"(n), "r"(bar) : "memory");
 }
-__device__ __forceinline__ float cv_act(float v, int act, float slope) {
-  switch (act) {
-    case 1: return fmaxf(v, 0.f);
-    case 2: return v > 0.f ? v : v * slope;
-    case 3: return 1.0f / (1.0f + expf(-v));
-    case 4: return tanhf(v);
-    default: return v;
-  }
+template <int BN>
+__device__ __forceinline__ void cv_mma(float (&d)[BN / 2], uint64_t a, uint64_t b, int scale_d) {
+  if constexpr (BN == 32) wg_mma_ss_n32(d, a, b, scale_d);
+  else if constexpr (BN == 64) wg_mma_ss_n64(d, a, b, scale_d);
+  else wg_mma_ss_n128(d, a, b, scale_d);
 }
 
+template <int BN>
 __global__ void __launch_bounds__(CV_THREADS, 1) k_conv_umma(const __grid_constant__ CVParams p) {
   extern __shared__ __align__(1024) uint8_t cv_raw[];
   uint8_t* base = cv_raw + ((1024u - (ua_smem(cv_raw) & 1023u)) & 1023u);
   const int a_slot_bytes = p.KW * p.a_copy_bytes;
-  const int b_tap_bytes = p.BN * 128, b_slot_bytes = p.KW * b_tap_bytes;
+  const int b_tap_bytes = BN * 128, b_slot_bytes = p.KW * b_tap_bytes;
   uint8_t* sA = base;
   uint8_t* sB = sA + p.na * a_slot_bytes;
   uint8_t* tail = base + p.ring_bytes;
-  // barriers: [0,na) a_full  [8,8+na) a_empty  [16,16+nb) b_full  [24,24+nb) b_empty  32 acc_full
+  // barriers: [0,na) a_full  [8,8+na) a_empty  [16,16+nb) b_full  [24,24+nb) b_empty
   unsigned long long* bars = reinterpret_cast<unsigned long long*>(tail);
-  uint32_t* tmem_base_p = reinterpret_cast<uint32_t*>(tail + 40 * 8);
   const uint32_t b0 = ua_smem(bars);
   auto bar = [&](int i) { return b0 + 8u * (uint32_t)i; };
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int tile = blockIdx.x, n0 = blockIdx.y * p.BN;
+  const int tile = blockIdx.x, n0 = blockIdx.y * BN;
   const int tpi = p.tiles_x * p.tiles_y;
   const int img = tile / tpi, trem = tile - img * tpi;
   const int y0 = (trem / p.tiles_x) * p.BH, x0 = (trem % p.tiles_x) * p.BW;
-  const int tmem_cols = p.BN < 32 ? 32 : p.BN;
+  const int nwg = p.M >> 6;                                       // consumer warpgroups with pixels to compute
 
   if (tid == 0) {
-    for (int i = 0; i < p.na; ++i) { ua_bar_init(bar(i), 1); ua_bar_init(bar(8 + i), 1); }
-    for (int i = 0; i < p.nb; ++i) { ua_bar_init(bar(16 + i), 1); ua_bar_init(bar(24 + i), 1); }
-    ua_bar_init(bar(32), 1);
+    for (int i = 0; i < p.na; ++i) { ua_bar_init(bar(i), 1); ua_bar_init(bar(8 + i), 4 * nwg); }
+    for (int i = 0; i < p.nb; ++i) { ua_bar_init(bar(16 + i), 1); ua_bar_init(bar(24 + i), 4 * nwg); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 5) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(ua_smem(tmem_base_p)), "r"(tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tD = *tmem_base_p;
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation, parameter / descriptor fetch) touches no
-  // global memory and overlaps the tail of the previous kernel in the stream; the next kernel may start its own prologue
-  // now.  Global reads and writes below wait for the previous grid to have completed and flushed.
+  // Programmatic dependent launch: everything above (barrier init, parameter / descriptor fetch) touches no global memory
+  // and overlaps the tail of the previous kernel in the stream; the next kernel may start its own prologue now.  Global
+  // reads and writes below wait for the previous grid to have completed and flushed.
   asm volatile("griddepcontrol.launch_dependents;");
   asm volatile("griddepcontrol.wait;" ::: "memory");
 
-  // The producer and MMA warps run their loops with all 32 lanes converged and hand single instructions to one elected
-  // lane (elect.sync): TMA and tcgen05 instructions execute on the uniform datapath, and inside a divergent `if (lane == 0)`
-  // region the compiler wraps every one of them in an ELECT / BRA.U.ANY loop and keeps the descriptor arithmetic in vector
-  // registers (R2UR per operand) -- measured here at ~100 issue cycles per MMA against 32-64 cycles of tensor-pipe work.
-  if (warp == 4) {
-    // ================================================= TMA producer
+  if (warp == 8) {
+    // ================================================= TMA producer: all 32 lanes stay converged, one elected lane issues
     int seg = 0, cb = 0, kbase = 0;                                  // kbase: first real k-block of the current segment
-    long long wa = 0, wb = 0, t1;
-    (void)wa; (void)wb; (void)t1;
-    CV_PROF(0, CV_CLK());
     for (int blk = 0; blk < p.nblk; ++blk) {
       const int sa = blk % p.na;
-      t1 = CV_CLK();
       ua_bar_wait(bar(8 + sa), ((blk / p.na) & 1) ^ 1);
-      wa += CV_CLK() - t1;
       if (ua_elect()) {
         cv_expect_tx(bar(sa), (uint32_t)a_slot_bytes);
         for (int dx = 0; dx < p.KW; ++dx)
@@ -154,9 +121,7 @@ __global__ void __launch_bounds__(CV_THREADS, 1) k_conv_umma(const __grid_consta
       __syncwarp();
       for (int dy = 0; dy < p.KH; ++dy) {
         const int ib = blk * p.KH + dy, sb = ib % p.nb;
-        t1 = CV_CLK();
         ua_bar_wait(bar(24 + sb), ((ib / p.nb) & 1) ^ 1);
-        wb += CV_CLK() - t1;
         if (ua_elect()) {
           cv_expect_tx(bar(16 + sb), (uint32_t)b_slot_bytes);
           for (int dx = 0; dx < p.KW; ++dx)
@@ -167,150 +132,103 @@ __global__ void __launch_bounds__(CV_THREADS, 1) k_conv_umma(const __grid_consta
       }
       if (++cb == p.seg_blocks[seg]) { cb = 0; kbase += p.seg_kblocks[seg]; ++seg; }
     }
-    if (lane == 0) { CV_PROF(1, wa); CV_PROF(2, wb); CV_PROF(3, CV_CLK()); }
-  } else if (warp == 5) {
-    // ================================================= MMA issuer
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(p.BN >> 3) << 17) | ((uint32_t)(p.M >> 4) << 24);
-    uint32_t acc = 0;
-    long long wa = 0, wb = 0, t1, tfirst = 0;
-    (void)wa; (void)wb; (void)t1; (void)tfirst;
-    if (lane == 0) CV_PROF(4, CV_CLK());
-    for (int blk = 0; blk < p.nblk; ++blk) {
-      const int sa = blk % p.na;
-      t1 = CV_CLK();
-      ua_bar_wait(bar(sa), (blk / p.na) & 1);
-      wa += CV_CLK() - t1;
-      if (blk == 0) tfirst = CV_CLK();
-      const uint64_t a_desc0 = ua_desc(ua_smem(sA + sa * a_slot_bytes));
-      for (int dy = 0; dy < p.KH; ++dy) {
-        const int ib = blk * p.KH + dy, sb = ib % p.nb;
-        t1 = CV_CLK();
-        ua_bar_wait(bar(16 + sb), (ib / p.nb) & 1);
-        wb += CV_CLK() - t1;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t b_desc0 = ua_desc(ua_smem(sB + sb * b_slot_bytes));
-        if (ua_elect()) {
-          // descriptors advance in their 16-byte address field: +2 per 8-float k-step, + tap / row offsets >> 4
-          uint64_t ad = a_desc0 + (uint64_t)((dy * p.BW * 128) >> 4), bd = b_desc0;
-          for (int dx = 0; dx < p.KW; ++dx) {
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              ua_mma_ss(tD, ad + 2 * ks, bd + 2 * ks, idesc, acc);
-              acc = 1;
-            }
-            ad += (uint64_t)(p.a_copy_bytes >> 4); bd += (uint64_t)(b_tap_bytes >> 4);
-          }
-          ua_commit(bar(24 + sb));
-          if (dy == p.KH - 1) ua_commit(bar(8 + sa));
-          if (dy == p.KH - 1 && blk == p.nblk - 1) ua_commit(bar(32));
-        }
-        acc = 1;
-        __syncwarp();
-      }
-    }
-    if (lane == 0) { CV_PROF(5, wa); CV_PROF(6, wb); CV_PROF(7, tfirst); CV_PROF(8, CV_CLK()); }
-  } else {
-    // ================================================= epilogue.  tcgen05.ld hands every thread one accumulator row (TMEM lane =
-    // pixel) x 32 columns; storing that way makes each warp instruction touch 32 different 128-byte lines (measured: ~2.2 k
-    // cycles of LSU wavefronts per 32 columns, and the same again for each of pre / res).  The rows therefore go through a
-    // 32 x 36-float staging tile per warp (the operand ring is idle by now) and the bias / pre / activation / residual math
-    // runs in the transposed mapping lane <-> (row = 4i + lane/8, 4 columns = lane%8): 8 lanes cover one pixel's 128 bytes,
-    // so every global load and store instruction moves four full lines.
-    const uint32_t lane_off = (uint32_t)(warp * 32) << 16;
-    const int rsub = lane >> 3, c4 = lane & 7;
-    const float* __restrict__ bias = p.bias;
-    const int act = p.act, post_relu = p.post_relu, round_tf32 = p.round_tf32;
-    const float slope = p.slope;
-    // M = 128: warp w's 32 TMEM lanes hold accumulator rows 32w .. 32w+31; M = 64: rows 16w .. 16w+15 in lanes 0-15 (the
-    // "half subpartition" layout of cta_group::1 M=64 accumulators, cute/atom/mma_traits_sm100.hpp), lanes 16-31 unused.
-    // The row pointers of this lane's 8 rows (row = 4i + lane/8) are built here, while the MMAs still run: the epilogue is
-    // one warp per scheduler, so every instruction of its dependent address arithmetic costs ~4 cycles of latency, and
-    // computing them per 32-column chunk (~1000 instructions with the 64-bit index math) was 2.4 k cycles per chunk.
-    const int rpw = p.M >> 2, bw_shift = p.BW == 16 ? 4 : 3;
-    const float* prow[8]; const float* rrow[8]; float* orow[8];
-    unsigned okmask = 0;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int rl = 4 * i + rsub, r = warp * rpw + rl;
-      const int y = y0 + (r >> bw_shift), x = x0 + (r & (p.BW - 1));
-      const bool ok = rl < rpw && y < p.H && x < p.W;
-      const long pix = ok ? ((long)img * p.H + y) * p.W + x : 0;
-      okmask |= ok ? (1u << i) : 0u;
-      orow[i] = p.out + pix * p.ld_out + n0 + 4 * c4;
-      prow[i] = p.pre ? p.pre + pix * p.ld_pre + n0 + 4 * c4 : nullptr;
-      rrow[i] = p.res ? p.res + pix * p.ld_res + n0 + 4 * c4 : nullptr;
-      asm volatile("" : "+l"(orow[i]), "+l"(prow[i]), "+l"(rrow[i]));        // keep them materialised here (no sinking into the loop)
-    }
-    const bool has_pre = p.pre != nullptr, has_res = p.res != nullptr;
-    const int nchunk = p.BN >> 5;
-    float* stgw = reinterpret_cast<float*>(sA) + warp * nchunk * (32 * 36);      // this warp's staging tiles, one per 32 columns
-    ua_bar_wait(bar(32), 0);
-    if (tid == 0) CV_PROF(9, CV_CLK());
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // Phase A: all TMEM loads first.  tcgen05.wait::ld also waits for the thread's outstanding global stores (measured with
-    // profiles/probes/umma_rate_probe.cu: 55 cycles with nothing in flight, 150-900 right after a burst of STG), so a
-    // load -> store -> load -> store sequence pays one store round trip per 32 columns.
-    for (int ch = 0; ch < nchunk; ++ch) {
-      uint32_t v[32];
-      UA_LD32(tD + ch * 32 + lane_off, v);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      float* stg = stgw + ch * (32 * 36);
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<float4*>(stg + lane * 36 + 4 * j) =
-            make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-    }
-    __syncwarp();
-    if (tid == 0) CV_PROF(12, CV_CLK());
-    // Phase B: bias / pre / activation / residual on the transposed mapping, coalesced loads and stores
-    for (int ch = 0; ch < nchunk; ++ch) {
-      const int n = n0 + ch * 32 + 4 * c4;
-      const bool n_in = n < p.Cout;
-      const float* stg = stgw + ch * (32 * 36);
-      float4 bv = make_float4(0.f, 0.f, 0.f, 0.f), pv[8], rv[8];
-      if (bias && n_in) bv = __ldg(reinterpret_cast<const float4*>(bias + n));
-      const unsigned on = n_in ? okmask : 0u;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        pv[i] = (has_pre && ((on >> i) & 1)) ? *reinterpret_cast<const float4*>(prow[i] + ch * 32) : make_float4(0.f, 0.f, 0.f, 0.f);
-        rv[i] = (has_res && ((on >> i) & 1)) ? *reinterpret_cast<const float4*>(rrow[i] + ch * 32) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      // the activation is selected once per chunk (warp-uniform branch), not per element: with the switch inside the
-      // element loop ptxas inlined the exp / tanh paths 32 times per chunk (~260 instructions between each shared-memory
-      // load and its global store; 3.8 k cycles per chunk measured)
-      // branch-free over the 8 rows (all shared-memory loads first, predicated stores last): with an `if (valid)` around
-      // each row the compiler serialised load -> ~50 dependent instructions -> store eight times (2.4 k cycles per chunk
-      // on four warps, measured), although the rows are independent
-      auto finish = [&](auto actf) {
-        float4 a[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) a[i] = *reinterpret_cast<const float4*>(stg + (4 * i + rsub) * 36 + 4 * c4);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          a[i].x = actf(a[i].x + (bv.x + pv[i].x)) + rv[i].x; a[i].y = actf(a[i].y + (bv.y + pv[i].y)) + rv[i].y;
-          a[i].z = actf(a[i].z + (bv.z + pv[i].z)) + rv[i].z; a[i].w = actf(a[i].w + (bv.w + pv[i].w)) + rv[i].w;
-          if (post_relu) { a[i].x = fmaxf(a[i].x, 0.f); a[i].y = fmaxf(a[i].y, 0.f); a[i].z = fmaxf(a[i].z, 0.f); a[i].w = fmaxf(a[i].w, 0.f); }
-          if (round_tf32) {
-            a[i].x = __uint_as_float(pp_tf32(a[i].x)); a[i].y = __uint_as_float(pp_tf32(a[i].y));
-            a[i].z = __uint_as_float(pp_tf32(a[i].z)); a[i].w = __uint_as_float(pp_tf32(a[i].w));
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          if ((on >> i) & 1) *reinterpret_cast<float4*>(orow[i] + ch * 32) = a[i];
-      };
-      if (act == 0) finish([](float v) { return v; });
-      else if (act == 1) finish([](float v) { return fmaxf(v, 0.f); });
-      else if (act == 2) finish([slope](float v) { return v > 0.f ? v : v * slope; });
-      else if (act == 3) finish([](float v) { return 1.0f / (1.0f + expf(-v)); });
-      else finish([](float v) { return tanhf(v); });
-    }
-    if (tid == 0) CV_PROF(14, CV_CLK());
+    return;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (tid == 0) CV_PROF(10, CV_CLK());
-  if (warp == 5) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tD), "r"(tmem_cols));
+  const int wg = warp >> 2;
+  if (wg >= nwg) return;                                          // 64-pixel tiles: the second warpgroup has no rows
+  // ================================================= consumer warpgroup: wgmma issue, then the epilogue from registers
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  // Each (block, dy) step is one wgmma group.  With two or more slots in both rings a slot is released one group late
+  // (wait_group 1), so the next group's wgmmas are issued before the previous ones retire; a one-slot ring is released at
+  // once (the producer could otherwise not fill the slot the next group waits for).
+  const bool defer = p.na >= 2 && p.nb >= 2;
+  int prev_sa = -1, prev_sb = -1;
+  const uint32_t row_off = (uint32_t)wg * 64 * 128;               // this warpgroup's 64 pixel rows inside every A copy
+  for (int blk = 0; blk < p.nblk; ++blk) {
+    const int sa = blk % p.na;
+    ua_bar_wait(bar(sa), (blk / p.na) & 1);
+    const uint64_t a_desc0 = ua_desc(ua_smem(sA + sa * a_slot_bytes) + row_off);
+    for (int dy = 0; dy < p.KH; ++dy) {
+      const int ib = blk * p.KH + dy, sb = ib % p.nb;
+      ua_bar_wait(bar(16 + sb), (ib / p.nb) & 1);
+      const uint64_t b_desc0 = ua_desc(ua_smem(sB + sb * b_slot_bytes));
+      // descriptors advance in their 16-byte address field: +2 per 8-float k-step, + tap / row offsets >> 4
+      uint64_t ad = a_desc0 + (uint64_t)((dy * p.BW * 128) >> 4), bd = b_desc0;
+      wg_fence();
+      for (int dx = 0; dx < p.KW; ++dx) {
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) cv_mma<BN>(acc, ad + 2 * ks, bd + 2 * ks, 1);
+        ad += (uint64_t)(p.a_copy_bytes >> 4); bd += (uint64_t)(b_tap_bytes >> 4);
+      }
+      wg_commit();
+      const int last_a = dy == p.KH - 1 ? sa : -1;
+      if (defer) {
+        wg_wait<1>();
+        if (prev_sb >= 0 && lane == 0) {
+          ua_bar_arrive(bar(24 + prev_sb));
+          if (prev_sa >= 0) ua_bar_arrive(bar(8 + prev_sa));
+        }
+        prev_sb = sb; prev_sa = last_a;
+      } else {
+        wg_wait<0>();
+        if (lane == 0) {
+          ua_bar_arrive(bar(24 + sb));
+          if (last_a >= 0) ua_bar_arrive(bar(8 + last_a));
+        }
+      }
+    }
+  }
+  wg_wait<0>();
+  wg_pin(acc);
+
+  // ================================================= epilogue straight from the accumulator registers: each thread owns
+  // two pixel rows x (2 adjacent channels per 8-channel group); a warp's float2 accesses cover whole 32-byte sectors.
+  const int g = lane >> 2, t = lane & 3;
+  const float* __restrict__ bias = p.bias;
+  const int post_relu = p.post_relu, round_tf32 = p.round_tf32;
+  const float slope = p.slope;
+  const float* prow[2]; const float* rrow[2]; float* orow[2];
+  bool ok[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = wg * 64 + (warp & 3) * 16 + g + 8 * h;
+    const int y = y0 + r / p.BW, x = x0 + r % p.BW;
+    ok[h] = y < p.H && x < p.W;
+    const long pix = ok[h] ? ((long)img * p.H + y) * p.W + x : 0;
+    orow[h] = p.out + pix * p.ld_out + n0 + 2 * t;
+    prow[h] = p.pre ? p.pre + pix * p.ld_pre + n0 + 2 * t : nullptr;
+    rrow[h] = p.res ? p.res + pix * p.ld_res + n0 + 2 * t : nullptr;
+  }
+  // the activation is selected once (warp-uniform branch), not per element: with the switch inside the element loop the
+  // exp / tanh paths would be inlined once per element
+  auto finish = [&](auto actf) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int n = n0 + 8 * j + 2 * t;
+      if (n >= p.Cout) continue;                                  // Cout % 4 == 0: n < Cout implies n + 1 < Cout
+      const float2 bv = bias ? __ldg(reinterpret_cast<const float2*>(bias + n)) : make_float2(0.f, 0.f);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!ok[h]) continue;
+        const float2 pv = prow[h] ? *reinterpret_cast<const float2*>(prow[h] + 8 * j) : make_float2(0.f, 0.f);
+        const float2 rv = rrow[h] ? *reinterpret_cast<const float2*>(rrow[h] + 8 * j) : make_float2(0.f, 0.f);
+        float2 a;
+        a.x = actf(acc[4 * j + 2 * h] + (bv.x + pv.x)) + rv.x;
+        a.y = actf(acc[4 * j + 2 * h + 1] + (bv.y + pv.y)) + rv.y;
+        if (post_relu) { a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f); }
+        if (round_tf32) { a.x = __uint_as_float(pp_tf32(a.x)); a.y = __uint_as_float(pp_tf32(a.y)); }
+        *reinterpret_cast<float2*>(orow[h] + 8 * j) = a;
+      }
+    }
+  };
+  const int act = p.act;
+  if (act == 0) finish([](float v) { return v; });
+  else if (act == 1) finish([](float v) { return fmaxf(v, 0.f); });
+  else if (act == 2) finish([slope](float v) { return v > 0.f ? v : v * slope; });
+  else if (act == 3) finish([](float v) { return 1.0f / (1.0f + expf(-v)); });
+  else finish([](float v) { return tanhf(v); });
 }
 
 // launch with the programmatic-stream-serialization attribute (PDL); PP_PDL=0 in the environment falls back to plain launches
@@ -357,9 +275,9 @@ static int cv_plan(const PPConvParams* q, CVParams* p, int* smem_bytes) {
     p->seg_kblocks[s] = (q->seg[s].C + 31) / 32;
     kblocks += p->seg_kblocks[s];
   }
-  // 1x1 convs (plain GEMMs over the channels): a pipeline stage of one 32-channel block holds only 4 MMAs, and the fixed
-  // cost of a stage (barrier round trip, tcgen05 fence, commits: ~300-900 cycles measured) then exceeds the MMAs' own
-  // ~290 cycles.  Group 4 consecutive blocks per stage (the tap loop walks channels instead of x-shifts).
+  // 1x1 convs (plain GEMMs over the channels): a pipeline stage of one 32-channel block holds only 4 wgmmas per warpgroup,
+  // less work than the fixed cost of a stage (two barrier round trips, a wgmma group commit and wait).  Group 4 consecutive
+  // blocks per stage (the tap loop walks channels instead of x-shifts).
   const int kv = (q->KH == 1 && q->KW == 1 && kblocks >= 8) ? 4 : 0;
   p->kgroup = kv ? 1 : 0;
   for (int s = 0; s < q->nseg; ++s) {
@@ -380,22 +298,23 @@ static int cv_plan(const PPConvParams* q, CVParams* p, int* smem_bytes) {
     const long a8 = (long)((q->W + 7) / 8) * ((q->H + mm / 8 - 1) / (mm / 8)), a16 = (long)((q->W + 15) / 16) * ((q->H + mm / 16 - 1) / (mm / 16));
     bw = a16 < a8 ? 16 : 8;
   }
-  const int M = q->tile_m == 64 ? 64 : 128;                      // UMMA M (pixels per CTA); 64 halves the per-MMA A traffic and the CTA's work
+  const int M = q->tile_m == 64 ? 64 : 128;                      // pixels per CTA = 64 per consumer warpgroup
   p->M = M;
   p->BW = bw; p->BH = M / bw;
   p->tiles_x = (q->W + p->BW - 1) / p->BW; p->tiles_y = (q->H + p->BH - 1) / p->BH;
   const long tiles = (long)p->tiles_x * p->tiles_y * q->n;
   if (tiles > 0x7fffffffL) return PP_ERR_SHAPE;
-  // N tile.  Measured with the CV_PROFILE counters (profiles/conv_prof.py): one M=128 kind::tf32 MMA with both operands in
-  // shared memory costs ~85 + 0.23*N cycles (the 128 x 32-byte A slices are read at ~48 B/clk whatever N is), and a CTA
-  // runs K/8 of them back to back; CTAs beyond one per SM run as further waves.  Pick the N that minimises
-  // waves x (85 + 0.23 N); ties go to the larger tile (fewer re-reads of A from L2).
+  // N tile.  Model of one k-step of 8 channels for the CTA's two warpgroups (m64nNk8 each, both operands in shared memory):
+  // the tensor cores need ~N cycles (1024 TF32 FMA per cycle per SM) and shared memory delivers the 2 x 2 KB A slices plus
+  // 2 x N x 32 B of B at 128 B per cycle, ~32 + N/2 cycles; the larger bounds the step.  One CTA runs per SM (shared
+  // memory), CTAs beyond one per SM run as further waves.  Pick the N that minimises waves x step cost; ties go to the
+  // larger tile (fewer re-reads of A from L2).
   int bn = q->bn;
   if (bn != 32 && bn != 64 && bn != 128) {
     long best = -1;
     for (int cand = 128; cand >= 32; cand >>= 1) {
       const long ctas = tiles * ((q->Cout + cand - 1) / cand), waves = (ctas + PP_NUM_SMS - 1) / PP_NUM_SMS;
-      const long cost = waves * (850 + 23 * cand / 10);
+      const long cost = waves * (cand > 32 + cand / 2 ? cand : 32 + cand / 2);
       if (best < 0 || cost < best) { best = cost; bn = cand; }
     }
   }
@@ -413,7 +332,6 @@ static int cv_plan(const PPConvParams* q, CVParams* p, int* smem_bytes) {
   while (na < CV_MAX_A_SLOTS && na < nblk && (na + 1) * a_slot + nb * b_slot <= CV_SMEM_BUDGET) ++na;
   p->na = na; p->nb = nb;
   p->ring_bytes = na * a_slot + nb * b_slot;
-  if (p->ring_bytes < 4 * (bn / 32) * 32 * 36 * 4) p->ring_bytes = 4 * (bn / 32) * 32 * 36 * 4;   // epilogue staging tiles
   *smem_bytes = p->ring_bytes + 512 + 1024;
   p->Cout = q->Cout;
   p->bias = q->bias; p->pre = q->pre; p->res = q->res; p->out = q->out;
@@ -462,13 +380,11 @@ extern "C" int pp_conv2d_umma(const PPConvParams* q, cudaStream_t stream) {
             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return PP_ERR_LAUNCH;
   }
-  if (cudaFuncSetAttribute(k_conv_umma, cudaFuncAttributeMaxDynamicSharedMemorySize, CV_SMEM_BUDGET + 2048) != cudaSuccess)
+  void (*kernel)(const CVParams) = p.BN == 32 ? k_conv_umma<32> : p.BN == 64 ? k_conv_umma<64> : k_conv_umma<128>;
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CV_SMEM_BUDGET + 2048) != cudaSuccess)
     return PP_ERR_LAUNCH;
-#ifdef CV_PROFILE
-  p.prof = g_cv_prof;
-#endif
   dim3 grid((unsigned)(p.tiles_x * p.tiles_y * p.n), (unsigned)((p.Cout + p.BN - 1) / p.BN));
-  if (cv_launch(k_conv_umma, grid, dim3(CV_THREADS), (size_t)smem, stream, p) != cudaSuccess) return PP_ERR_LAUNCH;
+  if (cv_launch(kernel, grid, dim3(CV_THREADS), (size_t)smem, stream, p) != cudaSuccess) return PP_ERR_LAUNCH;
   return cudaPeekAtLastError() == cudaSuccess ? PP_OK : PP_ERR_LAUNCH;
 }
 

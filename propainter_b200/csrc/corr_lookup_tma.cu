@@ -1,4 +1,4 @@
-// RAFT correlation lookup, TMA-staged (sm_100a).
+// RAFT correlation lookup, TMA-staged (sm_90a).
 //
 // One warp per source pixel.  For each of the 4 pyramid levels the warp's elected lane issues one
 // cp.async.bulk.tensor (TMA, 3-D tiled: x, y, plane) that lands the 16x10 neighbourhood of the lookup

@@ -1,4 +1,4 @@
-// HBM/L2-bound gather, stencil and elementwise kernels of the ProPainter hot path (sm_100a).
+// HBM/L2-bound gather, stencil and elementwise kernels of the ProPainter hot path (sm_90a).
 // One thread (or one warp) per output element; the per-element rules live in pp_elem.cuh.
 #include <stdlib.h>
 #include "pp_elem.cuh"

@@ -1,4 +1,4 @@
-// Common definitions for the propainter_b200 sm_100a kernels.
+// Common definitions for the propainter_b200 sm_90a kernels.
 //
 // Layout conventions (DESIGN.md §3):
 //   * "planar"  : [n][c][H][W]   -- tensors that cross the reference API boundary (frames, flows, masks)
@@ -44,4 +44,16 @@ static inline float4 make_float4(float a, float b, float c, float d) { float4 r 
 #define PP_DIV(a, b) ((a) / (b))
 #endif
 
-#define PP_NUM_SMS 148
+#if !defined(PP_HOSTSIM)
+// SM count of the current device, queried once (132 if none answers)
+static inline int pp_num_sms() {
+  static int n = 0;
+  int dev = 0;
+  if (n < 1 && (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1)) {
+    cudaGetLastError();
+    n = 132;
+  }
+  return n;
+}
+#define PP_NUM_SMS pp_num_sms()
+#endif

@@ -1,10 +1,6 @@
-// tcgen05 / TMEM / mbarrier building blocks (sm_100a) shared by the kernels that run on the 5th-generation tensor cores.
-// Every encoding here was validated in isolation on B200 with profiles/probes/umma_probe.cu:
-//   * K-major SWIZZLE_128B shared-memory operand descriptors (variant 0) and A operands read from TMEM (variant 3)
-//   * MN-major SWIZZLE_128B_BASE32B descriptors for 32-bit operands (variants 5/6; the plain SWIZZLE_128B layout is not
-//     accepted for MN-major tf32 and silently yields zeros)
-//   * kind::tf32 instruction descriptor, tcgen05.commit -> mbarrier, tcgen05.ld/st 32x32b
-// All waits are bounded and trap instead of hanging.
+// wgmma / mbarrier building blocks (sm_90a); operands K-major SWIZZLE_128B (TF32 wgmma needs K-major).  Accumulator of
+// m64nN: warp w holds rows 16w + g, 16w + g + 8 (g = lane / 4), columns 8j + 2(lane % 4) + {0, 1} in d[4j + {0,1} / {2,3}].
+// All mbarrier waits are bounded and trap instead of hanging.
 #pragma once
 #include <cstdint>
 
@@ -15,17 +11,6 @@ __device__ __forceinline__ void ua_bar_init(uint32_t bar, int count) {
 __device__ __forceinline__ void ua_bar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ bool ua_bar_test(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-               : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-  return done != 0;
-}
-__device__ __forceinline__ float ua_ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 __device__ __forceinline__ void ua_bar_wait(uint32_t bar, uint32_t parity) {
   uint32_t done = 0;
   for (int spin = 0; spin < (1 << 26) && !done; ++spin)
@@ -33,45 +18,54 @@ __device__ __forceinline__ void ua_bar_wait(uint32_t bar, uint32_t parity) {
                  : "=r"(done) : "r"(bar), "r"(parity) : "memory");
   if (!done) __trap();
 }
-// one lane of the (converged) warp: lets ptxas keep tcgen05 / TMA operands in uniform registers and predicate the single
+// one lane of the (converged) warp: lets ptxas keep TMA operands in uniform registers and predicate the single
 // instruction, instead of looping over the active lanes of a divergent region
 __device__ __forceinline__ bool ua_elect() {
   uint32_t pred = 0;
   asm volatile("{ .reg .b32 r; .reg .pred p; elect.sync r|p, 0xffffffff; selp.u32 %0, 1, 0, p; }" : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void ua_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// K-major SWIZZLE_128B shared-memory matrix descriptor (version 1, LBO unused = 16 B, SBO = 1024 B between 8-row groups)
+// K-major SWIZZLE_128B shared-memory matrix descriptor (LBO unused = 16 B, SBO = 1024 B between 8-row groups, layout 1 = 128B swizzle)
 __device__ __forceinline__ uint64_t ua_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 // byte offset of element (row, k) in a K-major SW128 tile with `rows` rows: k-block (32 floats) major, 8-row groups of 1 KB
 __device__ __forceinline__ uint32_t ua_off(int row, int k, int rows) {
   const int kb = k >> 5, kk = k & 31, r = row & 7;
   return (uint32_t)(kb * rows * 128 + (row >> 3) * 1024 + r * 128 + (((kk >> 2) ^ r) << 4) + (kk & 3) * 4);
 }
-__device__ __forceinline__ void ua_mma_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile("{ .reg .pred p; setp.ne.b32 p, %4, 0; tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p; }"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// wgmma writes its accumulator registers asynchronously: pin them around wg_wait with wg_pin (an empty volatile asm per
+// register), so the compiler does not move their reads or writes across the wait; issue wg_fence() before the next wgmma.
+template <int R>
+__device__ __forceinline__ void wg_pin(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void ua_mma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile("{ .reg .pred p; setp.ne.b32 p, %4, 0; tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p; }"
-               ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
+#define WG_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+__device__ __forceinline__ void wg_mma_ss_n32(float (&d)[16], uint64_t a, uint64_t b, int scale_d) {
+  asm volatile("{ .reg .pred p; setp.ne.b32 p, %18, 0; wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1; }"
+               : WG_D8(0), WG_D8(8)
+               : "l"(a), "l"(b), "r"(scale_d));
 }
-#define UA_LD32(taddr, v)                                                                                                    \
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];" \
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),   \
-                 "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),    \
-                 "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),    \
-                 "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])                                                                       \
-               : "r"(taddr))
-#define UA_ST32(taddr, v)                                                                                                    \
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" \
-               ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),  \
-                 "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), \
-                 "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), \
-                 "r"(v[30]), "r"(v[31]) : "memory")
 
+__device__ __forceinline__ void wg_mma_ss_n64(float (&d)[32], uint64_t a, uint64_t b, int scale_d) {
+  asm volatile("{ .reg .pred p; setp.ne.b32 p, %34, 0; wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1; }"
+               : WG_D8(0), WG_D8(8), WG_D8(16), WG_D8(24)
+               : "l"(a), "l"(b), "r"(scale_d));
+}
+
+__device__ __forceinline__ void wg_mma_ss_n128(float (&d)[64], uint64_t a, uint64_t b, int scale_d) {
+  asm volatile("{ .reg .pred p; setp.ne.b32 p, %66, 0; wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1; }"
+               : WG_D8(0), WG_D8(8), WG_D8(16), WG_D8(24), WG_D8(32), WG_D8(40), WG_D8(48), WG_D8(56)
+               : "l"(a), "l"(b), "r"(scale_d));
+}
+
+__device__ __forceinline__ void wg_mma_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t b, int scale_d) {
+  asm volatile("{ .reg .pred p; setp.ne.b32 p, %69, 0; wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1; }"
+               : WG_D8(0), WG_D8(8), WG_D8(16), WG_D8(24), WG_D8(32), WG_D8(40), WG_D8(48), WG_D8(56)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d));
+}

@@ -1,4 +1,4 @@
-"""One long clip across several GPUs (one process per GPU, torch.distributed; NCCL over NVLink on B200, gloo in the CPU tests).
+"""One long clip across several GPUs (one process per GPU, torch.distributed; NCCL over NVLink, gloo in the CPU tests).
 
 The reference's inference is single-device (SURVEY.md section 0.3); what it *does* have is a decomposition of every stage
 into independent units with recompute halos (inference_propainter.py:302-319, :342-364, :373-398, :417-452).  Those units

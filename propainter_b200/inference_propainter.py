@@ -10,7 +10,7 @@ from dataclasses import dataclass
 
 import torch
 
-from . import ops
+from . import config, ops
 from .model.modules.flow_comp_raft import RAFT_bi
 from .model.propainter import InpaintGenerator
 from .model.recurrent_flow_completion import RecurrentFlowCompleteNet
@@ -26,7 +26,8 @@ class InferenceConfig:
     # frames per RAFT call.  None = as many as an 8 GB correlation pyramid allows (never fewer than the reference's
     # 12/8/4/2, inference_propainter.py:302-309).  Frame pairs are independent, so this only changes batching.
     raft_clip_frames: int = None
-    windows_in_flight: int = 3      # generator windows computed concurrently on separate streams (compositing stays ordered)
+    # generator windows computed concurrently on side streams (compositing stays ordered); > 1 needs CUDA_GRAPHS off
+    windows_in_flight: int = 1
     # --fp16 (inference_propainter.py:211, :268-270, :323-330) halves the two nets and every tensor after RAFT.  The
     # kernels here compute in fp32 whatever the storage dtype (a `.half()` net is widened once, fp16 inputs are widened at
     # entry and results handed back in the caller's dtype), so the flag is accepted and changes nothing in the pipeline.
@@ -201,6 +202,10 @@ class ProPainterPipeline:
         in ascending window order because the 1/2-1/2 blend of inference_propainter.py:445-450 is order-dependent.
         jobs[k](slot) launches window k and returns its prediction."""
         nfl = max(1, int(cfg.windows_in_flight)) if cuda else 1
+        if nfl > 1 and config.CUDA_GRAPHS:
+            # concurrently replayed window graphs give a wrong, run-to-run different video (also with library convs and the
+            # mma.sync attention); run eagerly, windows in flight give exactly the one-at-a-time result
+            raise ValueError("windows_in_flight > 1 requires config.CUDA_GRAPHS = False")
         if nfl == 1:
             for k, jb in enumerate(jobs):
                 consume(k, jb(0))

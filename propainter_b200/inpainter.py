@@ -1,5 +1,5 @@
 """``ProInpainter``: the reference's high-level wrapper (web-demos/hugging_face/inpainter/base_inpainter.py:163-374) over the
-B200 pipeline.  Same constructor arguments and ``inpaint`` signature / result (list of uint8 frames at the output size);
+H100 pipeline.  Same constructor arguments and ``inpaint`` signature / result (list of uint8 frames at the output size);
 what differs is where the work happens: frame resizing (PIL BICUBIC), mask resizing (PIL NEAREST) + binarise + dilation
 (scipy binary_dilation), uint8 -> float conversion, the four inference stages, compositing and the output resize
 (cv2 INTER_LINEAR) all run on the device (propainter_b200.ops / ProPainterPipeline), so a call costs one host -> device

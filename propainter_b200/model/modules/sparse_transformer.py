@@ -1,4 +1,4 @@
-"""Soft split / composition and the mask-guided sparse temporal transformer (B200 execution plan).
+"""Soft split / composition and the mask-guided sparse temporal transformer (H100 execution plan).
 
 Reference: model/modules/sparse_transformer.py (SoftSplit :7-31, SoftComp :34-61, FusionFeedForward
 :64-101, SparseWindowAttention :117-281, TemporalSparseTransformer(Block) :284-344).  Parameters live in

@@ -1,5 +1,5 @@
 """``InpaintGenerator``: image propagation, encoder, flow-guided deformable feature propagation,
-mask-guided sparse transformer, decoder -- B200 execution plan.
+mask-guided sparse transformer, decoder -- H100 execution plan.
 
 Drop-in for the generator half of model/propainter.py (:256-372) of the reference: same constructor,
 ``img_propagation`` / ``forward`` signatures and results, same state_dict (216 tensors).  The GAN
@@ -118,7 +118,7 @@ class InpaintGenerator(ParamNet):
     def _feat_propagation(self, x, dsf, dsb, pmask, interpolation, gather_gemm=False):
         """BidirectionalPropagation(128, learnable=True).forward propainter.py:104-190.
         x [lt,h,w,128] pixel-major; dsf/dsb [lt-1,h,w,2]; pmask [lt,h,w,2] -> fused [lt,128,h,w].
-        gather_gemm: the deformable conv as pp_deform_gather + one 1x1 tcgen05 GEMM over the sampled columns instead of
+        gather_gemm: the deformable conv as pp_deform_gather + one 1x1 wgmma GEMM over the sampled columns instead of
         the tap pre-pass + split-K mma.sync kernel + reduce (the library convs around it stay)."""
         if interpolation != "bilinear":
             raise NotImplementedError("the feature propagation path uses bilinear warping (propainter.py:319 default)")
@@ -165,7 +165,7 @@ class InpaintGenerator(ParamNet):
         z = conv(as_nchw(z), self._wb(fp + "fuse.0", 2 * C + 4), 1, 1, act="leaky", slope=0.2)
         return conv(z, self._wb(fp + "fuse.2"), 1, 1, res=as_nchw(x))
 
-    # ---- the same scan on the tcgen05 conv kernel (config.UMMA_CONV)
+    # ---- the same scan on the wgmma conv kernel (config.UMMA_CONV)
     def _uw(self, key, sel, segs):
         """packed weight of conv `key` restricted to the input channels `sel` (list of (lo, hi)) split into segments `segs`"""
         def build():
@@ -177,7 +177,7 @@ class InpaintGenerator(ParamNet):
         return self.P[key + ".bias"]
 
     def _feat_propagation_umma(self, x, dsf, dsb, pmask):
-        """`_feat_propagation` with every conv of the scan on pp_conv2d_umma (tcgen05, TF32 products, fused bias /
+        """`_feat_propagation` with every conv of the scan on pp_conv2d_umma (wgmma, TF32 products, fused bias /
         activation / residual / placement epilogues, multi-segment inputs instead of concat buffers) and the deformable
         conv as pp_deform_gather + a 1x1 pp_conv2d_umma.  Only the part of each conv that depends on the recurrent state
         stays inside the sequential loop: conv(cat[a, b]) = conv_a(a) + conv_b(b), so the shares of conv_offset.0 and
@@ -252,7 +252,7 @@ class InpaintGenerator(ParamNet):
         conv_b(b), so the shares of conv_offset.0 and backbone.0 over step-independent inputs (current frame, flow, validity,
         mask: 133 of 261 and 130 of 258 input channels) are one batched conv per scan, and the per-step convs see only the
         128 state-dependent channels (K = 1152 instead of 2376 / 2340); their result enters through pp_bias_act_pre.  The
-        deformable conv is pp_deform_gather + a 1x1 tcgen05 GEMM."""
+        deformable conv is pp_deform_gather + a 1x1 wgmma GEMM."""
         lt, h, w, C = x.shape
         dev = x.device
         fp = "feat_prop_module."

@@ -1,4 +1,4 @@
-"""Recurrent flow completion network on the B200 hot path.
+"""Recurrent flow completion network on the H100 hot path.
 
 Drop-in for model/recurrent_flow_completion.py:203-347 of the reference (constructor, ``forward``,
 ``forward_bidirect_flow``, ``combine_flow``, state_dict incl. the training-only edge head).
@@ -77,7 +77,7 @@ class RecurrentFlowCompleteNet(ParamNet):
 
     def _propagate(self, x, gather_gemm=False):
         """BidirectionalPropagation.forward :67-124.  x [t,128,h,w] channels_last -> same.
-        gather_gemm: deformable conv = pp_deform_gather + one 1x1 tcgen05 GEMM (library convs around it unchanged)."""
+        gather_gemm: deformable conv = pp_deform_gather + one 1x1 wgmma GEMM (library convs around it unchanged)."""
         t, c, h, w = x.shape
         dev = x.device
         xs = as_pm(x)                                                         # [t,h,w,128]
@@ -130,7 +130,7 @@ class RecurrentFlowCompleteNet(ParamNet):
         return self.packed(f"uw:{key}:{sel}:{segs}", build)
 
     def _propagate_umma(self, x):
-        """`_propagate` on the tcgen05 conv kernel (config.UMMA_CONV): every conv of the scan is one pp_conv2d_umma launch
+        """`_propagate` on the wgmma conv kernel (config.UMMA_CONV): every conv of the scan is one pp_conv2d_umma launch
         with its bias / LeakyReLU / residual / placement fused, the two previous states are read as two input segments straight
         from the history buffer (no torch.cat), the deformable conv is pp_deform_gather (split input) + a 1x1 conv over the
         sampled columns, and the shares of conv_offset.0 / backbone.0 that only see the current frame (and, in the forward

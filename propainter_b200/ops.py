@@ -145,7 +145,7 @@ def deform_align(x, o, flow, max_res, w_packed, bias, out, o_bias=None):
 
 
 def tf32_round(w):
-    """fp32 -> nearest TF32 value (ties away from zero, = cvt.rna.tf32.f32), still stored as fp32.  tcgen05 kind::tf32
+    """fp32 -> nearest TF32 value (ties away from zero, = cvt.rna.tf32.f32), still stored as fp32.  wgmma kind tf32
     ignores the low 13 mantissa bits; rounding once at pack time keeps the products unbiased."""
     i = w.contiguous().view(torch.int32)
     return ((i + 0x1000) & ~0x1FFF).view(torch.float32)
@@ -178,7 +178,7 @@ def _pm4(t):
 
 def conv_umma(segs, w_packed, KH, KW, Cout, bias=None, act="none", slope=0.0, pre=None, res=None, post_relu=False, out=None,
               round_tf32=False, bn=0, tile_w=0, tile_m=0):
-    """tcgen05 implicit-GEMM conv (stride 1, same padding) with fused epilogue.  segs: list of [n,H,W,C_i] pixel-major
+    """wgmma implicit-GEMM conv (stride 1, same padding) with fused epilogue.  segs: list of [n,H,W,C_i] pixel-major
     views = the channel-concatenated input; w_packed from pack_conv_weight(weight, [C_i...]); pre / res / out
     [n,H,W,Cout] views (channel slices of wider buffers allowed).  Returns out."""
     n, H, W, _ = segs[0].shape
@@ -295,7 +295,7 @@ def window_mask(pmask, fh, fw, nwh, nww):
 
 def sparse_window_attn(qkv, pool_kv, key_tok, flags, t, NT, kf_start, kf_step, out=None, WN=45, C=512, impl="umma"):
     """qkv [t,NT,3C]; pool_kv [t,NP,2C]; key_tok int32 [nwin,NKO]; flags int32 [nwin] -> out [t,NT,C].
-    impl: "umma" = tcgen05/TMEM kernel for masked windows (default), "mma" = warp-level mma.sync baseline."""
+    impl: "umma" = wgmma kernel for masked windows (default), "mma" = warp-level mma.sync baseline."""
     if out is None:
         out = torch.empty(t, NT, C, device=qkv.device, dtype=torch.float32)
     prm = PPAttnParams()

@@ -85,8 +85,8 @@ def test_flow_completion_matches_oracle():
 @pytest.mark.parametrize("plan", [0, 1, 2, 3, 4])
 def test_every_scan_plan_matches_oracle(plan, monkeypatch):
     """The propagation scans exist as several numerically equivalent plans and autotune.pick replays whichever measures
-    fastest, so a timing flip must never change the result class: force each candidate in turn (0 all tcgen05 convs, 1
-    library convs + mma.sync deformable kernel, 2 library convs + gather / tcgen05 GEMM, 3 / 4 the same with the frame-only
+    fastest, so a timing flip must never change the result class: force each candidate in turn (0 all wgmma convs, 1
+    library convs + mma.sync deformable kernel, 2 library convs + gather / wgmma GEMM, 3 / 4 the same with the frame-only
     conv shares hoisted; the generator has 4 candidates) and compare both nets with the oracle."""
     from propainter_b200 import autotune, config
     from propainter_b200.model.propainter import InpaintGenerator
@@ -314,3 +314,19 @@ def test_proinpainter_wrapper_matches_host_pre_post_processing():
     ref = np.stack([cv2.resize(f, out_size) for f in comp])
     d = np.abs(got.astype(int) - ref.astype(int))
     assert d.max() <= 1 and (d > 0).mean() < 1e-3, (d.max(), (d > 0).mean())
+
+
+@pytest.mark.shipping
+def test_windows_in_flight_bit_identical(monkeypatch):
+    """Concurrent windows (graphs off) give exactly the one-at-a-time video; with graphs on they are refused."""
+    from propainter_b200 import config, synth
+    from propainter_b200.inference_propainter import InferenceConfig, ProPainterPipeline
+    u8, fm, md = synth.make_clip(40, 240, 432, mask="ellipse", seed=0)
+    pipe = ProPainterPipeline(device=DEV)
+    x = torch.from_numpy(u8)
+    with pytest.raises(ValueError):
+        pipe(x, fm, md, InferenceConfig(windows_in_flight=3))
+    monkeypatch.setattr(config, "CUDA_GRAPHS", False)
+    one = pipe(x, fm, md, InferenceConfig(windows_in_flight=1)).cpu().numpy()
+    for _ in range(2):
+        assert np.array_equal(pipe(x, fm, md, InferenceConfig(windows_in_flight=3)).cpu().numpy(), one)

@@ -182,7 +182,7 @@ def test_deform_align():
 
 
 def test_conv_umma_matches_torch_conv():
-    """pp_conv2d_umma (tcgen05 implicit GEMM, TMA-staged shifted halo boxes) vs F.conv2d in fp32.  `exact`: operands that are
+    """pp_conv2d_umma (wgmma implicit GEMM, TMA-staged shifted halo boxes) vs F.conv2d in fp32.  `exact`: operands that are
     exactly representable in TF32, so every product is exact and only the fp32 accumulation order differs (1e-5 of the
     output scale: any indexing / swizzle / segment-order mistake is O(1)); `plain`: arbitrary fp32 activations reach the
     tensor core truncated to TF32 (3e-3 of the output scale; 1.7e-3 measured at K = 1280)."""

@@ -5,7 +5,7 @@
     these clips (tests/golden/make_golden.py, ~10 min of CPU each in the authoring container): RAFT flows, completed flows,
     propagated frames / masks (8x-subsampled) and the composited uint8 video inside the holes (outside them the video is the
     input, which is checked bit-exactly).  The shipping defaults (TF32 tensor-core products, CUDA graphs, autotuned plans)
-    are compared stage by stage; bars are ~10x the error measured on B200 (printed by the test).
+    are compared stage by stage (the errors are printed by the test).
   * the oracle itself is pinned at full size by running it on the GPU in strict fp32 against the same golden.
   * size-independent properties (zero mask = identity, replay determinism, the hole never grows)."""
 import os
@@ -62,8 +62,6 @@ def test_full_size_vs_reference_golden(key):
     print(f"{key}: " + " ".join(f"{k}={v:.2e}" for k, v in e.items()) +
           f" | PSNR {psnr:.2f} dB (holes only {psnr_hole:.2f} dB), max |diff| {d.max()}, >1 level: {(d > 1).mean():.2e}")
     assert np.array_equal(a[~hole], u8[~hole])
-    # measured on B200 (round 2): flows 1.4e-3 / 1.5e-3 (TF32 library convs in RAFT), masks and propagated frames exact,
-    # PSNR 72.1 dB (C2) / 67.2 dB (C3), 61.1 dB inside the holes, max |diff| 1 level
     assert e["gt_f"] < 1e-2 and e["gt_b"] < 1e-2 and e["pred_f"] < 1e-2 and e["pred_b"] < 1e-2
     assert e["upd_m_mismatch"] < 1e-3 and e["upd_f_mismatch"] < 1e-3
     assert psnr_hole > 52.0 and psnr > 60.0 and d.max() <= 4
