@@ -39,6 +39,16 @@ int pp_corr_lookup(const float* const* levels, const float* coords, float* out, 
 /* same contract, plain global loads instead of TMA staging (baseline for the ncu comparison) */
 int pp_corr_lookup_ldg(const float* const* levels, const float* coords, float* out, long n_pairs, int h, int w,
                        cudaStream_t stream);
+/* AlternateCorrBlock RAFT/corr.py:83-111 (the memory-free lookup behind args.alternate_corr, raft.py:44-45,106-109):
+ * levels 1-3 of the per-frame feature pyramid, 2x2 average pooling with avg_pool2d's floor sizes.  fmap pixel-major
+ * [frames][h*w][D] (D % 4 == 0); pooled: host array of 3 device pointers, pooled[l-1] = [frames][(h>>l)*(w>>l)][D]. */
+int pp_corr_fmap_pyramid(const float* fmap, int D, int frames, int h, int w, float* const* pooled, cudaStream_t stream);
+/* The lookup of AlternateCorrBlock: pair p correlates frame idx1[p] with idx2[p] of fmap (level 0) and pooled (levels
+ * 1-3, from pp_corr_fmap_pyramid) at lookup time; D = 256.  Writes the tensor of pp_corr_lookup -- coords
+ * [n_pairs*h*w][2] (x,y) -> out [n_pairs*h*w][324] -- with CorrBlock's channel order, /sqrt(D) scaling and sampling
+ * rule (corr.py:29-50, bilinear_sampler RAFT/utils/utils.py:57-71), so no volume of n_pairs*(h*w)^2 floats is stored. */
+int pp_corr_lookup_otf(const float* fmap, const float* const* pooled, int D, const int* idx1, const int* idx2, int n_pairs,
+                       const float* coords, float* out, int h, int w, cudaStream_t stream);
 /* RAFT.upsample_flow RAFT/raft.py:73-84.  mask pixel-major [n*h*w][ld_mask>=576] (unscaled conv output,
  * mask_scale = 0.25 from update.py:135); flow_lr [n][h][w][2]; out planar [n][2][8h][8w]. */
 int pp_convex_upsample(const float* mask, int ld_mask, float mask_scale, const float* flow_lr, float* out, int n,

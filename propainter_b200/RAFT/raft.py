@@ -7,6 +7,9 @@ What differs is the execution plan:
   * the all-pairs volume + pyramid (corr.py:13-27) is built by ``ops.corr_build`` (fp32-accurate
     3xTF32 tensor-core GEMM) into row-padded planes; the 4-level 9x9 lookup (corr.py:29-50) is one
     kernel writing the 324-channel pixel-major tensor the motion encoder consumes
+  * where that volume cannot fit the device, or with the reference's ``args.alternate_corr``, the on-the-fly plan
+    (AlternateCorrBlock, corr.py:83-111) pools the features instead and forms the window dot products at lookup time,
+    writing the same 324-channel tensor (``corr_plan`` below)
   * z and r gates of the SepConvGRU share one conv (concatenated weights); eval BatchNorm is folded
     into the cnet convs; the mask head + convex upsampling run only on the last iteration (the
     reference computes them 20x and keeps one, raft.py:135-146)
@@ -20,6 +23,47 @@ from .. import ops
 from .._params import ParamNet
 from ..nn_util import as_nchw, as_pm, cl, conv
 from ..schemas import raft_schema
+
+
+ALL_PAIRS, ON_THE_FLY = "all_pairs", "on_the_fly"
+# Bytes per input-frame pixel that one all-pairs RAFT call needs besides its correlation pyramid: encoder activations,
+# context / GRU buffers, the 324-channel lookup output, the upsampled flows.  Measured by profiles/raft_mem.py on an
+# H100 80GB HBM3 (700 W power limit): a 2-frame call (2 pairs, 20 iterations) peaked 2,676,002,816 bytes above its
+# inputs at 1280x720, of which 2,200,320,000 are the two pyramids -> 258.1 B per pixel of the 2 frames (257.3 at
+# 1920x1080).  Rounded up.
+RAFT_WS_BYTES_PER_PX = 260
+# Bytes per input-frame pixel that each pair of an on-the-fly call adds (the same buffers, no pyramid; the pooled
+# feature levels are ~1/3 of fmap): same tool and card, the peak of a 4-frame call (6 pairs) minus that of a
+# 2-frame call (2 pairs) over 4 pairs -> 243.6 B per pixel at 1280x720 and 1920x1080.  Rounded up.
+OTF_BYTES_PER_PAIR_PX = 244
+
+
+def pyramid_bytes(h, w):
+    """Bytes of the 4-level all-pairs correlation pyramid of one pair on an h x w feature grid (ops.corr_alloc)."""
+    n, hl, wl, total = h * w, h, w, 0
+    for _ in range(4):
+        total += n * hl * ops.corr_ld(wl) * 4
+        hl, wl = hl // 2, wl // 2
+    return total
+
+
+def corr_plan(H, W, alternate=False, total_bytes=None):
+    """The correlation plan of every RAFT call on H x W frames.  ON_THE_FLY (AlternateCorrBlock: no volume, the window
+    dot products formed at lookup time) when the caller asks for it -- the reference's `args.alternate_corr` -- or when
+    the smallest all-pairs call (2 frames: one pair per direction) with its working set exceeds the device's memory
+    `total_bytes` (None: no limit).  ALL_PAIRS otherwise: it is the faster plan wherever it fits, and every size that
+    runs all-pairs keeps its numerics."""
+    if alternate:
+        return ON_THE_FLY
+    if total_bytes is not None and 2 * pyramid_bytes(H // 8, W // 8) + RAFT_WS_BYTES_PER_PX * 2 * H * W > total_bytes:
+        return ON_THE_FLY
+    return ALL_PAIRS
+
+
+def device_bytes(device):
+    """Total memory of a CUDA device, None elsewhere."""
+    device = torch.device(device)
+    return torch.cuda.get_device_properties(device).total_memory if device.type == "cuda" else None
 
 
 class RAFT(ParamNet):
@@ -105,12 +149,21 @@ class RAFT(ParamNet):
         return fmap.view(n, h * w, d), net, inp, (h, w)
 
     # ------------------------------------------------------------------ refinement loop (raft.py:122-146)
-    def _refine(self, fmap, idx1, idx2, net, inp, hw, iters, flow_init=None):
+    def corr_plan(self, H, W, device):
+        """corr_plan for this net's `args` (reference flag `alternate_corr`) on `device`."""
+        return corr_plan(H, W, bool(getattr(self.args, "alternate_corr", False)), device_bytes(device))
+
+    def _refine(self, fmap, idx1, idx2, net, inp, hw, iters, plan, flow_init=None):
         h, w = hw
         B = idx1.numel()
         dev = fmap.device
-        levels = ops.corr_alloc(B, h, w, dev)
-        ops.corr_build(fmap, idx1, idx2, levels, h, w)
+        if plan == ON_THE_FLY:
+            pooled = ops.corr_fmap_pyramid(fmap, h, w)
+            lookup = lambda c, out: ops.corr_lookup_otf(fmap, pooled, idx1, idx2, c, out)
+        else:
+            levels = ops.corr_alloc(B, h, w, dev)
+            ops.corr_build(fmap, idx1, idx2, levels, h, w)
+            lookup = lambda c, out: ops.corr_lookup(levels, c, out)
         ys, xs = torch.meshgrid(torch.arange(h, device=dev), torch.arange(w, device=dev), indexing="ij")
         c0 = torch.stack([xs, ys], -1).float()[None].expand(B, h, w, 2).contiguous()     # coords_grid (utils.py:74-77)
         c1 = c0.clone()
@@ -133,7 +186,7 @@ class RAFT(ParamNet):
         mot_in = torch.empty(B, h, w, 256, device=dev)          # [cor(192) | flo(64)] without a torch.cat (update.py:95)
         mw, mb = self._motion_out()
         for _ in range(iters):
-            ops.corr_lookup(levels, c1, corr)
+            lookup(c1, corr)
             flow_pm = c1 - c0
             flow = as_nchw(flow_pm)
             cor = conv(as_nchw(corr), self._wb(u + "encoder.convc1"), act="relu")
@@ -161,21 +214,23 @@ class RAFT(ParamNet):
         if not test_mode:
             raise NotImplementedError("training-mode flow_predictions list is outside the inference hot path")
         n = image1.shape[0]
+        plan = self.corr_plan(image1.shape[-2], image1.shape[-1], image1.device)
         fmap, net, inp, hw = self.encode_frames(torch.cat([image1, image2], 0))
         idx1 = torch.arange(n, device=image1.device, dtype=torch.int32)
-        return self._refine(fmap, idx1, idx1 + n, net[:n], inp[:n], hw, iters, flow_init)
+        return self._refine(fmap, idx1, idx1 + n, net[:n], inp[:n], hw, iters, plan, flow_init)
 
     @torch.no_grad()
     def flows_bidirectional(self, frames, iters=20):
         """frames [l,3,H,W] -> (forward flows i->i+1, backward flows i+1->i), each [l-1,2,H,W].
         Encoders + 20 refinement iterations replay as one CUDA graph per clip shape."""
-        return self.graphs(("raft_bi", iters), lambda fr: self._flows_bidirectional(fr, iters), frames.contiguous())
+        plan = self.corr_plan(frames.shape[-2], frames.shape[-1], frames.device)
+        return self.graphs(("raft_bi", iters, plan), lambda fr: self._flows_bidirectional(fr, iters, plan), frames.contiguous())
 
-    def _flows_bidirectional(self, frames, iters):
+    def _flows_bidirectional(self, frames, iters, plan=ALL_PAIRS):
         l = frames.shape[0]
         fmap, net, inp, hw = self.encode_frames(frames)
         a = torch.arange(l - 1, device=frames.device, dtype=torch.int32)
         idx1, idx2 = torch.cat([a, a + 1]), torch.cat([a + 1, a])
         sel = idx1.long()
-        _, up = self._refine(fmap, idx1, idx2, net[sel], inp[sel], hw, iters)
+        _, up = self._refine(fmap, idx1, idx2, net[sel], inp[sel], hw, iters, plan)
         return up[:l - 1], up[l - 1:]

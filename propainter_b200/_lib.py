@@ -51,6 +51,8 @@ SIGNATURES = {
     "pp_corr_pool_pyramid": (c_int, [c_void_p, c_long, c_int, c_int, c_void_p]),
     "pp_corr_lookup": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_int, c_int, c_void_p]),
     "pp_corr_lookup_ldg": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_int, c_int, c_void_p]),
+    "pp_corr_fmap_pyramid": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "pp_corr_lookup_otf": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "pp_convex_upsample": (c_int, [c_void_p, c_int, c_float, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pp_img_prop_scan_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "pp_img_prop_scan": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_int,

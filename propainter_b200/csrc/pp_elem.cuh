@@ -198,6 +198,31 @@ PP_HD float pp_corr_tap(const float* plane, int Hl, int Wl, int ld, float cx, fl
   PPTaps t = pp_taps(pp_raft_coord(x, Wl), pp_raft_coord(y, Hl), Hl, Wl);
   return pp_tap_plane(plane, ld, t);
 }
+// AlternateCorrBlock (RAFT/corr.py:83-111) without a stored plane: level `lvl` is sampled from a 10x10 tile of dot
+// products, tile[j*10 + i] = f1 . f2_l[ty0 + j][tx0 + i] / sqrt(D) (zero outside the level), whose origin is the
+// floored level centre minus the window radius.  Far-away or non-finite centres get a tile wholly outside the level.
+PP_HD int pp_corr_tile_origin(float c, int lvl) {
+  float v = floorf(PP_DIV(c, (float)(1 << lvl)));
+  v = fminf(fmaxf(v, -1.0e6f), 1.0e6f);
+  return (int)v - 4;
+}
+// Tap (a, b) of level `lvl` from that tile by the rule of pp_corr_tap.  The grid_sample coordinate round trip can move
+// a corner by one step at an integer boundary; a corner that lands off the tile then weighs 0 or a few ulp and is dropped.
+PP_HD float pp_corr_tap_tile(const float* tile, int tx0, int ty0, int Hl, int Wl, float cx, float cy, int lvl, int a, int b) {
+  float s = (float)(1 << lvl);
+  float x = PP_ADD(PP_DIV(cx, s), (float)(a - 4));
+  float y = PP_ADD(PP_DIV(cy, s), (float)(b - 4));
+  PPTaps t = pp_taps(pp_raft_coord(x, Wl), pp_raft_coord(y, Hl), Hl, Wl);
+  if (!t.any) return 0.f;
+  const int i = t.x0 - tx0, j = t.y0 - ty0;
+  const bool i0 = i >= 0 && i < 10, i1 = i >= -1 && i < 9, j0 = j >= 0 && j < 10, j1 = j >= -1 && j < 9;
+  float acc = 0.f;
+  if (t.w00 != 0.f && j0 && i0) acc += tile[j * 10 + i] * t.w00;
+  if (t.w01 != 0.f && j0 && i1) acc += tile[j * 10 + i + 1] * t.w01;
+  if (t.w10 != 0.f && j1 && i0) acc += tile[(j + 1) * 10 + i] * t.w10;
+  if (t.w11 != 0.f && j1 && i1) acc += tile[(j + 1) * 10 + i + 1] * t.w11;
+  return acc;
+}
 
 // RAFT/raft.py:73-84: convex 8x upsampling of one low-res pixel's (i,j) sub-pixel.
 // mask pixel-major [..][576], channel k*64 + i*8 + j; flow_lr pixel-interleaved [h][w][2].

@@ -11,6 +11,7 @@ from dataclasses import dataclass
 import torch
 
 from . import config, ops
+from .RAFT.raft import ON_THE_FLY, OTF_BYTES_PER_PAIR_PX
 from .model.modules.flow_comp_raft import RAFT_bi
 from .model.propainter import InpaintGenerator
 from .model.recurrent_flow_completion import RecurrentFlowCompleteNet
@@ -56,6 +57,18 @@ def raft_clip_len(width):
         if width <= limit:
             return n
     return 2
+
+
+def auto_clip_frames(T, H, W, plan):
+    """Frames per RAFT call when InferenceConfig.raft_clip_frames is None: as many as fit an 8 GB budget for the
+    plan's per-pair memory (all-pairs: the 4-level pyramid, ~1.34 N^2 floats; on-the-fly: the lookup output, GRU
+    buffers and encoder activations, RAFT.OTF_BYTES_PER_PAIR_PX per input pixel), never fewer than the reference's."""
+    if plan == ON_THE_FLY:
+        pairs = int(8e9 // (OTF_BYTES_PER_PAIR_PX * H * W))
+    else:
+        n = (H // 8) * (W // 8)
+        pairs = int(8e9 // (5.4 * n * n))
+    return max(raft_clip_len(W), min(T, pairs // 2 + 1))
 
 
 def flow_chunks(T, clip):
@@ -122,9 +135,7 @@ class ProPainterPipeline:
         T, H, W = frames.shape[1], frames.shape[-2], frames.shape[-1]
         clip = cfg.raft_clip_frames
         if clip is None:
-            n = (H // 8) * (W // 8)
-            pairs = int(8e9 // (5.4 * n * n))                         # 4 pyramid levels ~ 1.34 N^2 floats per pair
-            clip = max(raft_clip_len(W), min(T, pairs // 2 + 1))
+            clip = auto_clip_frames(T, H, W, self.fix_raft.fix_raft.corr_plan(H, W, frames.device))
         ff, bb = [], []
         for s, e in flow_chunks(T, clip):
             f, b = self.fix_raft(frames[:, s:e], iters=cfg.raft_iter)

@@ -91,6 +91,32 @@ def corr_lookup(levels, coords, out=None, tma=True):
     return out
 
 
+def corr_fmap_pyramid(fmap, h, w):
+    """fmap [frames, h*w, D] pixel-major -> levels 1-3 of its per-frame 2x2 average-pooled pyramid, each
+    [frames, (h>>l)*(w>>l), D]: the stored half of the on-the-fly correlation (AlternateCorrBlock)."""
+    F_, _, D = fmap.shape
+    pooled = [torch.empty(F_, (h >> l) * (w >> l), D, device=fmap.device, dtype=torch.float32) for l in (1, 2, 3)]
+    check(_lib.lib().pp_corr_fmap_pyramid(_p(_dense(fmap)), D, F_, h, w, (ctypes.c_void_p * 3)(*[p.data_ptr() for p in pooled]),
+                                          _stream()), "pp_corr_fmap_pyramid")
+    _count(3)
+    return pooled
+
+
+def corr_lookup_otf(fmap, pooled, idx1, idx2, coords, out=None):
+    """corr_lookup without the all-pairs volume: pair p correlates frame idx1[p] with idx2[p] (int32 CUDA [n_pairs]) of
+    fmap [frames, h*w, 256] and its pooled levels (corr_fmap_pyramid) at lookup time.  coords [B,h,w,2] -> [B,h,w,324]."""
+    B, h, w, _ = coords.shape
+    if idx1.numel() != B or idx2.numel() != B:
+        raise RuntimeError("corr_lookup_otf: one (idx1, idx2) entry per coords batch row")
+    if out is None:
+        out = torch.empty(B, h, w, 324, device=coords.device, dtype=torch.float32)
+    levels = (ctypes.c_void_p * 3)(*[_p(_dense(p)).value for p in pooled])
+    check(_lib.lib().pp_corr_lookup_otf(_p(_dense(fmap)), levels, fmap.shape[-1], _p(idx1, torch.int32), _p(idx2, torch.int32), B,
+                                        _p(_dense(coords)), _p(_dense(out)), h, w, _stream()), "pp_corr_lookup_otf")
+    _count(1)
+    return out
+
+
 def convex_upsample(mask_pm, flow_lr, mask_scale=0.25):
     """mask_pm [n,h,w,576] pixel-major, flow_lr [n,h,w,2] -> planar [n,2,8h,8w]."""
     n, h, w, _ = flow_lr.shape
