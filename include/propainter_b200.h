@@ -234,6 +234,17 @@ typedef struct PPWindowIds { int n; int frame[PP_MAX_WINDOW]; int first[PP_MAX_W
  * ori/comp uint8 [T][H][W][3]; ids (host struct): target frame + first-visit flag per local frame. */
 int pp_composite_blend_u8(const float* pred, const float* masks, const uint8_t* ori, uint8_t* comp,
                           const PPWindowIds* ids, int H, int W, cudaStream_t stream);
+/* ---- video outpainting (inference_propainter.py --mode video_outpainting) --------------------------- */
+/* extrapolation inference_propainter.py:117-156 + to_tensors of its masks (:265-266): uint8 frames [T][h][w][3] are
+ * placed at (top, left) of a zero canvas [T][H][W][3]; flow_masks / masks_dilated float {0,1} [T][1][H][W] are 1 outside
+ * [top+rim_h, top+h-rim_h) x [left+rim_w, left+w-rim_w) and outside the source rectangle respectively (an empty range
+ * clears nothing, as numpy slicing does).  The reference's geometry: rim = 4 if offset > 10 else 0.
+ * PP_ERR_SHAPE unless the source rectangle lies inside the canvas and the rims are >= 0. */
+int pp_extrapolate_u8(const uint8_t* src, uint8_t* canvas, float* flow_masks, float* masks_dilated, int T, int h, int w, int H,
+                      int W, int top, int left, int rim_h, int rim_w, cudaStream_t stream);
+/* the masked-frame preview inference_propainter.py:250-261: per channel, in float64, fuse = 0.4*img + 0.6*(0,255,0),
+ * mask*fuse + (1-mask)*img, truncated to uint8.  frames uint8 [T][H][W][3], masks [T][1][H][W] -> out uint8 [T][H][W][3]. */
+int pp_mask_overlay_u8(const uint8_t* frames, const float* masks, uint8_t* out, int T, int H, int W, cudaStream_t stream);
 
 #ifdef __cplusplus
 }

@@ -102,6 +102,8 @@ SIGNATURES = {
                                          c_void_p]),
     "pp_composite_blend_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(PPWindowIds), c_int, c_int,
                                       c_void_p]),
+    "pp_extrapolate_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 9 + [c_void_p]),
+    "pp_mask_overlay_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
 }
 
 _lib = None

@@ -808,3 +808,56 @@ extern "C" int pp_composite_blend_u8(const float* pred, const float* masks, cons
   PP_LAUNCH_CHECK();
   return PP_OK;
 }
+
+// ================================================================ video outpainting + masked preview
+// One thread per canvas pixel: its 3 canvas bytes and its value in both masks.  64-bit offsets (a 3840x2160 canvas
+// holds 8.3 M pixels per frame).
+__global__ void __launch_bounds__(256) k_extrapolate_u8(const uint8_t* __restrict__ src, uint8_t* __restrict__ canvas,
+    float* __restrict__ flow_masks, float* __restrict__ masks_dilated, int T, int h, int w, int H, int W, int top,
+    int left, int rim_h, int rim_w) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;  // over T*H*W
+  const long HW = (long)H * W;
+  if (i >= (long)T * HW) return;
+  const long f = i / HW; const long p = i - f * HW; const int y = (int)(p / W), x = (int)(p - (long)y * W);
+  const long s = pp_outpaint_src(y, x, top, left, h, w);
+  uint8_t r = 0, g = 0, b = 0;
+  if (s >= 0) {
+    const uint8_t* sp = src + (f * h * w + s) * 3;
+    r = sp[0]; g = sp[1]; b = sp[2];
+  }
+  uint8_t* cp = canvas + i * 3;
+  cp[0] = r; cp[1] = g; cp[2] = b;
+  flow_masks[i] = pp_outpaint_mask(y, x, top, left, h, w, rim_h, rim_w);
+  masks_dilated[i] = pp_outpaint_mask(y, x, top, left, h, w, 0, 0);
+}
+// replaces extrapolation (inference_propainter.py:117-156) + to_tensors of its masks (:265-266): uint8 frames
+// [T][h][w][3] -> zero-bordered canvas [T][H][W][3] and float {0,1} flow / dilated masks [T][1][H][W]
+extern "C" int pp_extrapolate_u8(const uint8_t* src, uint8_t* canvas, float* flow_masks, float* masks_dilated, int T, int h,
+                                 int w, int H, int W, int top, int left, int rim_h, int rim_w, cudaStream_t stream) {
+  if (T < 1 || h < 1 || w < 1 || top < 0 || left < 0 || rim_h < 0 || rim_w < 0) return PP_ERR_SHAPE;
+  if ((long)top + h > H || (long)left + w > W) return PP_ERR_SHAPE;
+  const long n = (long)T * H * W;
+  k_extrapolate_u8<<<pp_blocks(n, 256), 256, 0, stream>>>(src, canvas, flow_masks, masks_dilated, T, h, w, H, W, top, left,
+                                                          rim_h, rim_w);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+
+__global__ void __launch_bounds__(256) k_mask_overlay_u8(const uint8_t* __restrict__ frames, const float* __restrict__ masks,
+                                                         uint8_t* __restrict__ out, int T, int H, int W) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;  // over T*H*W*3 (HWC order of the uint8 frames)
+  const long HW = (long)H * W;
+  if (i >= (long)T * HW * 3) return;
+  const long p = i / 3; const int c = (int)(i - p * 3);
+  out[i] = pp_mask_overlay(frames[i], masks[p], c);
+}
+// replaces the masked_frame_for_save loop of inference_propainter.py:250-261 (green overlay, alpha 0.6): frames uint8
+// [T][H][W][3] + masks [T][1][H][W] -> preview uint8 [T][H][W][3]
+extern "C" int pp_mask_overlay_u8(const uint8_t* frames, const float* masks, uint8_t* out, int T, int H, int W,
+                                  cudaStream_t stream) {
+  if (T < 1 || H < 1 || W < 1) return PP_ERR_SHAPE;
+  const long n = (long)T * H * W * 3;
+  k_mask_overlay_u8<<<pp_blocks(n, 256), 256, 0, stream>>>(frames, masks, out, T, H, W);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}

@@ -43,6 +43,16 @@ static inline float4 make_float4(float a, float b, float c, float d) { float4 r 
 #define PP_SUB(a, b) ((a) - (b))
 #define PP_DIV(a, b) ((a) / (b))
 #endif
+// the same for double, where a rule restates a float64 numpy expression bit for bit
+#if defined(__CUDA_ARCH__)
+#define PP_DMUL(a, b) __dmul_rn((a), (b))
+#define PP_DADD(a, b) __dadd_rn((a), (b))
+#define PP_DSUB(a, b) __dsub_rn((a), (b))
+#else
+#define PP_DMUL(a, b) ((a) * (b))
+#define PP_DADD(a, b) ((a) + (b))
+#define PP_DSUB(a, b) ((a) - (b))
+#endif
 
 #if !defined(PP_HOSTSIM)
 // SM count of the current device, queried once (132 if none answers)

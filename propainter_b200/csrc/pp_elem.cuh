@@ -318,3 +318,27 @@ PP_HD float pp_mask_dilate_pixel(const uint8_t* m, int H, int W, int y, int x, i
   }
   return 0.0f;
 }
+
+// ------------------------------------------------------------------------------------------------
+// Video outpainting (extrapolation, inference_propainter.py:117-156).  The h x w source sits at (top, left) of the
+// zero canvas; canvas pixel (y, x) shows source pixel pp_outpaint_src (-1: border, value 0).
+PP_HD long pp_outpaint_src(int y, int x, int top, int left, int h, int w) {
+  const int sy = y - top, sx = x - left;
+  return (sy >= 0 && sy < h && sx >= 0 && sx < w) ? (long)sy * w + sx : -1;
+}
+// Mask value of canvas pixel (y, x): 0 inside [top+rim_h, top+h-rim_h) x [left+rim_w, left+w-rim_w), 1 elsewhere
+// (:144-151).  rim (4 if offset > 10 else 0) gives the flow mask, rim 0 the dilated mask.  Like the numpy slice, an
+// empty range (h <= 2*rim_h) clears nothing.
+PP_HD float pp_outpaint_mask(int y, int x, int top, int left, int h, int w, int rim_h, int rim_w) {
+  const bool in = y >= top + rim_h && y < top + h - rim_h && x >= left + rim_w && x < left + w - rim_w;
+  return in ? 0.0f : 1.0f;
+}
+// Green preview of the masked region (inference_propainter.py:251-261), one channel c of one pixel, in float64 as numpy
+// computes it: fuse = (1-a)*img + a*green, mask*fuse + (1-mask)*img, astype(uint8) truncation; a = 0.6, green = (0,255,0).
+PP_HD uint8_t pp_mask_overlay(uint8_t img, float mask, int c) {
+  const double a = 0.6, v = (double)img, m = (double)mask;
+  const double green = c == 1 ? 255.0 : 0.0;
+  const double fuse = PP_DADD(PP_DMUL(PP_DSUB(1.0, a), v), PP_DMUL(a, green));
+  const double out = PP_DADD(PP_DMUL(m, fuse), PP_DMUL(PP_DSUB(1.0, m), v));
+  return (uint8_t)(int)out;
+}

@@ -6,6 +6,7 @@ on the device, and replaces the per-window ``.cpu()`` + numpy compositing (:437-
 so a clip needs exactly one host->device and one device->host copy.  Chunk boundaries, halo lengths,
 reference-frame selection and the order-dependent blend follow the reference exactly.
 """
+import math
 from dataclasses import dataclass
 
 import torch
@@ -105,6 +106,36 @@ def prepare_masks(masks_u8, mask_dilation=4, device="cuda"):
     m = masks_u8.to(device)
     d = ops.mask_dilate(m, mask_dilation).unsqueeze(0)
     return d, d.clone()
+
+
+def outpaint_geometry(h, w, scale_h, scale_w):
+    """extrapolation's geometry (inference_propainter.py:123-128, :142-143) for an h x w source:
+    ((H, W), (top, left), (rim_h, rim_w)) = the canvas, the source's offset in it and the flow-mask rim.
+
+    The reference's expressions in Python doubles: int(scale * size) rounded down to a multiple of 8, offset
+    int((H - h) / 2), rim 4 if offset > 10 else 0 (1.4 * 360 = 503.99999999999994 gives 496, not 504).  Deviation: a
+    canvas smaller than the source in either dimension, where the reference's negative offset makes the numpy slice
+    fail or misplace the frame, and a non-finite scale raise ValueError."""
+    sh, sw = float(scale_h), float(scale_w)
+    if not (math.isfinite(sh) and math.isfinite(sw)):
+        raise ValueError(f"outpainting scale must be finite, got ({scale_h}, {scale_w})")
+    H, W = int(sh * h), int(sw * w)
+    H, W = H - H % 8, W - W % 8
+    if H < h or W < w:
+        raise ValueError(f"outpainting canvas {H}x{W} is smaller than the {h}x{w} source (scale ({scale_h}, {scale_w}))")
+    top, left = int((H - h) / 2), int((W - w) / 2)
+    return (H, W), (top, left), (4 if top > 10 else 0, 4 if left > 10 else 0)
+
+
+def prepare_outpainting(frames_u8, scale_h=1.0, scale_w=1.2, device="cuda"):
+    """extrapolation (inference_propainter.py:117-156) + to_tensors of its masks (:265-266) on the device: uint8 frames
+    [T,h,w,3] (host or device) -> (canvas uint8 [T,H,W,3], flow_masks, masks_dilated float {0,1} [1,T,1,H,W], (W, H)),
+    the reference's return order and its --scale_h / --scale_w defaults (:206-209).  mask_dilation plays no part."""
+    src = torch.as_tensor(frames_u8).to(device).contiguous()
+    geo = outpaint_geometry(src.shape[1], src.shape[2], scale_h, scale_w)
+    canvas, fm, md = ops.extrapolate_u8(src, geo)
+    H, W = geo[0]
+    return canvas, fm.unsqueeze(0), md.unsqueeze(0), (W, H)
 
 
 class ProPainterPipeline:
@@ -260,3 +291,18 @@ class ProPainterPipeline:
         if return_stages:
             return comp, {"gt_flows": gt, "pred_flows": pred, "updated_frames": upd_f, "updated_masks": upd_m}
         return comp
+
+    @torch.no_grad()
+    def outpaint(self, frames_u8, scale_h=1.0, scale_w=1.2, cfg=None, return_stages=False):
+        """--mode video_outpainting (inference_propainter.py:243-246): prepare_outpainting, then the four stages on the
+        widened canvas.  frames_u8 uint8 [T,h,w,3] (host or device).  Returns the composited canvas uint8 [T,H,W,3] on
+        the device (the script's final cv2.resize to the source size, :469-470, is ops.resize_output_u8(comp, (w, h)))."""
+        canvas, flow_masks, masks_dilated, _ = prepare_outpainting(frames_u8, scale_h, scale_w, self.device)
+        return self(canvas, flow_masks, masks_dilated, cfg, return_stages)
+
+    def masked_preview(self, frames_u8, masks_dilated):
+        """The script's second video (inference_propainter.py:250-261), in either mode: the holes of `masks_dilated`
+        ([1,T,1,H,W] or [T,1,H,W] float) tinted green over uint8 frames [T,H,W,3].  Returns uint8 [T,H,W,3] on the device."""
+        dev = self.device
+        frames = torch.as_tensor(frames_u8).to(dev, non_blocking=True).contiguous()
+        return ops.mask_overlay_u8(frames, masks_dilated.to(dev, non_blocking=True).float().contiguous())

@@ -494,6 +494,40 @@ def composite_blend(pred, masks, ori_u8, comp_u8, frame_ids, first_flags):
     _count(1)
 
 
+def extrapolate_u8(frames_u8, geometry):
+    """extrapolation (inference_propainter.py:117-156) on the device: uint8 [T,h,w,3] and a geometry
+    ((H, W), (top, left), (rim_h, rim_w)) from inference_propainter.outpaint_geometry -> (canvas uint8 [T,H,W,3],
+    flow_masks float {0,1} [T,1,H,W], masks_dilated float {0,1} [T,1,H,W])."""
+    (H, W), (top, left), (rim_h, rim_w) = geometry
+    if frames_u8.dim() != 4 or frames_u8.shape[-1] != 3:
+        raise RuntimeError("extrapolate_u8: expected uint8 frames [T,h,w,3]")
+    T, h, w, _ = frames_u8.shape
+    src = _p(_dense(frames_u8), torch.uint8)
+    dev = frames_u8.device
+    canvas = torch.empty(T, H, W, 3, dtype=torch.uint8, device=dev)
+    fm = torch.empty(T, 1, H, W, dtype=torch.float32, device=dev)
+    md = torch.empty_like(fm)
+    check(_lib.lib().pp_extrapolate_u8(src, _p(canvas, torch.uint8), _p(fm), _p(md), T, h, w, H, W, top, left, rim_h, rim_w,
+                                       _stream()), "pp_extrapolate_u8")
+    _count(1)
+    return canvas, fm, md
+
+
+def mask_overlay_u8(frames_u8, masks):
+    """The green masked-frame preview of inference_propainter.py:250-261: uint8 [T,H,W,3] + float masks with T*H*W
+    elements ([T,1,H,W] or the pipeline's [1,T,1,H,W]) -> uint8 [T,H,W,3]."""
+    if frames_u8.dim() != 4 or frames_u8.shape[-1] != 3:
+        raise RuntimeError("mask_overlay_u8: expected uint8 frames [T,H,W,3]")
+    T, H, W, _ = frames_u8.shape
+    if masks.numel() != T * H * W or tuple(masks.shape[-2:]) != (H, W):
+        raise RuntimeError(f"mask_overlay_u8: masks {tuple(masks.shape)} do not match frames {tuple(frames_u8.shape)}")
+    out = torch.empty_like(frames_u8)
+    check(_lib.lib().pp_mask_overlay_u8(_p(_dense(frames_u8), torch.uint8), _p(_dense(masks)), _p(out, torch.uint8), T, H, W,
+                                        _stream()), "pp_mask_overlay_u8")
+    _count(1)
+    return out
+
+
 # ---------------------------------------------------------------- resizing around the path (tables on the host, passes on the device)
 _TABLES = {}
 
