@@ -1,5 +1,6 @@
 """Tensor-level wrappers over the C ABI.  Each takes/returns torch CUDA tensors, passes raw pointers +
 the current stream, and raises on any non-zero return code.  fp32 only (DESIGN.md §6)."""
+import collections
 import ctypes
 import math
 
@@ -202,27 +203,28 @@ def _pm4(t):
     return _pm(t)
 
 
-def conv_umma(segs, w_packed, KH, KW, Cout, bias=None, act="none", slope=0.0, pre=None, res=None, post_relu=False, out=None,
-              round_tf32=False, bn=0, tile_w=0, tile_m=0):
-    """wgmma implicit-GEMM conv (stride 1, same padding) with fused epilogue.  segs: list of [n,H,W,C_i] pixel-major
-    views = the channel-concatenated input; w_packed from pack_conv_weight(weight, [C_i...]); pre / res / out
-    [n,H,W,Cout] views (channel slices of wider buffers allowed).  Returns out."""
-    n, H, W, _ = segs[0].shape
-    if out is None:
-        out = torch.empty(n, H, W, Cout, device=segs[0].device, dtype=torch.float32)
+def _conv_params(segs, KH, KW, Cout, w_packed=None, bias=None, act="none", slope=0.0, pre=None, res=None, post_relu=False,
+                 out=None, round_tf32=False, bn=0, tile_w=0, tile_m=0):
+    """PPConvParams of one pp_conv2d_umma call (see conv_umma).  A segment may also be given as its shape (n, H, W, C):
+    its pointer is then null and its ld is C rounded up to a multiple of 4 (the narrowest buffer conv_umma accepts), which
+    is enough for pp_conv2d_umma_plan."""
+    if not 1 <= len(segs) <= _lib.PP_CONV_MAX_SEG:
+        raise RuntimeError(f"conv_umma: {len(segs)} input segments (1 to {_lib.PP_CONV_MAX_SEG} supported)")
+    shapes = [tuple(s.shape) if isinstance(s, torch.Tensor) else tuple(s) for s in segs]
+    n, H, W, _ = shapes[0]
     prm = PPConvParams()
     prm.nseg = len(segs)
     kblocks = 0
-    for i, sgm in enumerate(segs):
-        if tuple(sgm.shape[:3]) != (n, H, W):
+    for i, (sgm, shp) in enumerate(zip(segs, shapes)):
+        if len(shp) != 4 or shp[:3] != (n, H, W):
             raise RuntimeError("conv_umma: segment shape mismatch")
-        ptr, ld = _pm4(sgm)
-        prm.seg[i].x, prm.seg[i].ld, prm.seg[i].C = ptr.value, ld, sgm.shape[-1]
-        kblocks += (sgm.shape[-1] + 31) // 32
-    if tuple(w_packed.shape) != (Cout, kblocks * KH * KW * 32):
+        ptr, ld = _pm4(sgm) if isinstance(sgm, torch.Tensor) else (ctypes.c_void_p(None), (shp[3] + 3) // 4 * 4)
+        prm.seg[i].x, prm.seg[i].ld, prm.seg[i].C = ptr.value, ld, shp[3]
+        kblocks += (shp[3] + 31) // 32
+    if w_packed is not None and tuple(w_packed.shape) != (Cout, kblocks * KH * KW * 32):
         raise RuntimeError(f"conv_umma: packed weight {tuple(w_packed.shape)} does not match {(Cout, kblocks * KH * KW * 32)}")
     prm.n, prm.H, prm.W, prm.KH, prm.KW = n, H, W, KH, KW
-    prm.w_packed, prm.Cout = _p(_dense(w_packed)).value, Cout
+    prm.w_packed, prm.Cout = _p(_dense(w_packed)).value if w_packed is not None else None, Cout
     prm.bias = _p(bias).value if bias is not None else None
     for name, t in (("pre", pre), ("res", res), ("out", out)):
         if t is None:
@@ -236,9 +238,34 @@ def conv_umma(segs, w_packed, KH, KW, Cout, bias=None, act="none", slope=0.0, pr
         setattr(prm, "ld_" + name, ld)
     prm.act, prm.slope, prm.post_relu, prm.round_tf32 = ACT[act], float(slope), int(bool(post_relu)), int(bool(round_tf32))
     prm.bn, prm.tile_w, prm.tile_m = int(bn), int(tile_w), int(tile_m)
+    return prm
+
+
+def conv_umma(segs, w_packed, KH, KW, Cout, bias=None, act="none", slope=0.0, pre=None, res=None, post_relu=False, out=None,
+              round_tf32=False, bn=0, tile_w=0, tile_m=0):
+    """wgmma implicit-GEMM conv (stride 1, same padding) with fused epilogue.  segs: list of [n,H,W,C_i] pixel-major
+    views = the channel-concatenated input; w_packed from pack_conv_weight(weight, [C_i...]); pre / res / out
+    [n,H,W,Cout] views (channel slices of wider buffers allowed).  Returns out."""
+    if out is None and segs:
+        n, H, W, _ = segs[0].shape
+        out = torch.empty(n, H, W, Cout, device=segs[0].device, dtype=torch.float32)
+    prm = _conv_params(segs, KH, KW, Cout, w_packed, bias, act, slope, pre, res, post_relu, out, round_tf32, bn, tile_w, tile_m)
     check(_lib.lib().pp_conv2d_umma(ctypes.byref(prm), _stream()), "pp_conv2d_umma")
     _count(1)
     return out
+
+
+ConvPlan = collections.namedtuple("ConvPlan", "tile_h tile_w bn ctas smem_bytes")
+
+
+def conv_plan(segs, KH, KW, Cout, bn=0, tile_w=0, tile_m=0, out=None, pre=None, res=None, bias=None):
+    """The tile / ring plan conv_umma would launch for these arguments (pp_conv2d_umma_plan), without launching it:
+    ConvPlan(tile_h, tile_w, bn, ctas, smem_bytes).  segs as in conv_umma, or their shapes (n, H, W, C_i).  Raises where
+    conv_umma would refuse the plan."""
+    prm = _conv_params(segs, KH, KW, Cout, bias=bias, pre=pre, res=res, out=out, bn=bn, tile_w=tile_w, tile_m=tile_m)
+    vals = [ctypes.c_int(0) for _ in range(5)]
+    check(_lib.lib().pp_conv2d_umma_plan(ctypes.byref(prm), *[ctypes.byref(v) for v in vals]), "pp_conv2d_umma_plan")
+    return ConvPlan(*[v.value for v in vals])
 
 
 def deform_gather(x, o, flow, max_res, cols=None, o_bias=None, x2=None):
