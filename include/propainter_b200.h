@@ -245,6 +245,18 @@ int pp_extrapolate_u8(const uint8_t* src, uint8_t* canvas, float* flow_masks, fl
 /* the masked-frame preview inference_propainter.py:250-261: per channel, in float64, fuse = 0.4*img + 0.6*(0,255,0),
  * mask*fuse + (1-mask)*img, truncated to uint8.  frames uint8 [T][H][W][3], masks [T][1][H][W] -> out uint8 [T][H][W][3]. */
 int pp_mask_overlay_u8(const uint8_t* frames, const float* masks, uint8_t* out, int T, int H, int W, cudaStream_t stream);
+/* ---- optical-flow colour coding (RAFT/utils/flow_viz.py, RAFT/utils/flow_viz_pt.py) ------------------- */
+#define PP_FLOWVIZ_FRAME 0 /* flow_viz.py::flow_to_image per frame: rad_max + 1e-5, numpy >= 2 dtypes, rad > 1 -> x0.75 */
+#define PP_FLOWVIZ_CLIP 1  /* flow_viz_pt.py::flow_to_image: max_norm + FLT_EPSILON over the whole batch, float32 */
+/* Group maxima of sqrt(u^2 + v^2) over planar float32 flow [N][2][H][W], after np.clip(flow, 0, clip_flow) when
+ * has_clip: maxima[N] (per_frame = 1) or maxima[1] (per_frame = 0), caller-owned; cleared on the stream first.
+ * PP_ERR_SHAPE unless 1 <= N <= 65535 and H, W >= 1. */
+int pp_flow_maxrad(const float* flow, float* maxima, int N, int H, int W, int per_frame, int has_clip, float clip_flow,
+                   cudaStream_t stream);
+/* The colour wheel of `variant` (PP_FLOWVIZ_*) over the same flow (clipped when has_clip), normalised by the maxima of
+ * pp_flow_maxrad with the matching per_frame -> uint8 out [N][H][W][3], RGB (BGR when bgr). */
+int pp_flow_to_image_u8(const float* flow, const float* maxima, uint8_t* out, int N, int H, int W, int variant, int has_clip,
+                        float clip_flow, int bgr, cudaStream_t stream);
 
 #ifdef __cplusplus
 }

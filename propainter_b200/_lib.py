@@ -104,6 +104,8 @@ SIGNATURES = {
                                       c_void_p]),
     "pp_extrapolate_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 9 + [c_void_p]),
     "pp_mask_overlay_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "pp_flow_maxrad": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [ctypes.c_float, c_void_p]),
+    "pp_flow_to_image_u8": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [ctypes.c_float, c_int, c_void_p]),
 }
 
 _lib = None

@@ -861,3 +861,67 @@ extern "C" int pp_mask_overlay_u8(const uint8_t* frames, const float* masks, uin
   PP_LAUNCH_CHECK();
   return PP_OK;
 }
+
+// ================================================================ optical-flow colour coding
+// Planar flow [N][2][H][W] float32 -> uint8 [N][H][W][3].  Two HBM-bound passes: the group maxima of the (clipped)
+// radius (8 B read per pixel), then one thread per pixel (8 B read, 3 B written).  64-bit offsets: a 4K clip's output
+// passes 2^31 bytes.
+__global__ void __launch_bounds__(256) k_flow_maxrad(const float* __restrict__ flow, float* __restrict__ maxima, long HW,
+                                                     int per_frame, int has_clip, float clip_flow) {
+  const int n = blockIdx.y;
+  const float* u = flow + (long)n * 2 * HW;
+  const float* v = u + HW;
+  float m = 0.0f;
+  for (long p = (long)blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += (long)gridDim.x * blockDim.x) {
+    float a = __ldg(u + p), b = __ldg(v + p);
+    if (has_clip) { a = pp_flow_clip(a, clip_flow); b = pp_flow_clip(b, clip_flow); }
+    m = fmaxf(m, pp_flow_rad(a, b));
+  }
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  __shared__ float red[8];
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 1; i < 8; ++i) m = fmaxf(m, red[i]);
+    // a non-negative float orders like its bit pattern, so the integer max is the float max, in any order
+    atomicMax((int*)(maxima + (per_frame ? n : 0)), __float_as_int(m));
+  }
+}
+// the per-frame rad_max of flow_viz.py:127-128 (per_frame = 1, maxima[N]) or the batch max_norm of flow_viz_pt.py:29
+// (per_frame = 0, maxima[1]); clears the maxima on the stream first
+extern "C" int pp_flow_maxrad(const float* flow, float* maxima, int N, int H, int W, int per_frame, int has_clip,
+                              float clip_flow, cudaStream_t stream) {
+  if (N < 1 || N > 65535 || H < 1 || W < 1) return PP_ERR_SHAPE;
+  const long HW = (long)H * W;
+  if (cudaMemsetAsync(maxima, 0, (per_frame ? N : 1) * sizeof(float), stream) != cudaSuccess) return PP_ERR_LAUNCH;
+  const int bx = pp_blocks(HW, 256 * 8) < 512 ? pp_blocks(HW, 256 * 8) : 512;
+  k_flow_maxrad<<<dim3(bx, N), 256, 0, stream>>>(flow, maxima, HW, per_frame, has_clip, clip_flow);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+
+__global__ void __launch_bounds__(256) k_flow_to_image_u8(const float* __restrict__ flow, const float* __restrict__ maxima,
+                                                          uint8_t* __restrict__ out, int N, long HW, int variant,
+                                                          int has_clip, float clip_flow, int bgr) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;  // over N*H*W
+  if (i >= (long)N * HW) return;
+  const long n = i / HW, p = i - n * HW;
+  float u = __ldg(flow + n * 2 * HW + p), v = __ldg(flow + n * 2 * HW + HW + p);
+  if (has_clip) { u = pp_flow_clip(u, clip_flow); v = pp_flow_clip(v, clip_flow); }
+  uint8_t rgb[3];
+  if (variant == PP_FLOWVIZ_FRAME) pp_flowviz_np(u, v, PP_ADD(__ldg(maxima + n), 1e-5f), bgr, rgb);
+  else pp_flowviz_pt(u, v, PP_ADD(__ldg(maxima), 1.1920928955078125e-07f), bgr, rgb);
+  uint8_t* o = out + i * 3;
+  o[0] = rgb[0]; o[1] = rgb[1]; o[2] = rgb[2];
+}
+// replaces RAFT/utils/flow_viz.py::flow_to_image per frame (PP_FLOWVIZ_FRAME, maxima[N] from pp_flow_maxrad) and
+// flow_viz_pt.py::flow_to_image over the batch (PP_FLOWVIZ_CLIP, maxima[1]), written pixel-major
+extern "C" int pp_flow_to_image_u8(const float* flow, const float* maxima, uint8_t* out, int N, int H, int W, int variant,
+                                   int has_clip, float clip_flow, int bgr, cudaStream_t stream) {
+  if (N < 1 || H < 1 || W < 1) return PP_ERR_SHAPE;
+  if (variant != PP_FLOWVIZ_FRAME && variant != PP_FLOWVIZ_CLIP) return PP_ERR_SHAPE;
+  const long HW = (long)H * W, n = (long)N * HW;
+  k_flow_to_image_u8<<<pp_blocks(n, 256), 256, 0, stream>>>(flow, maxima, out, N, HW, variant, has_clip, clip_flow, bgr != 0);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}

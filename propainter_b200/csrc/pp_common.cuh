@@ -53,6 +53,14 @@ static inline float4 make_float4(float a, float b, float c, float d) { float4 r 
 #define PP_DADD(a, b) ((a) + (b))
 #define PP_DSUB(a, b) ((a) - (b))
 #endif
+// correctly rounded square root and float64 division (the flow colour rules)
+#if defined(__CUDA_ARCH__)
+#define PP_SQRT(a) __fsqrt_rn(a)
+#define PP_DDIV(a, b) __ddiv_rn((a), (b))
+#else
+#define PP_SQRT(a) sqrtf(a)
+#define PP_DDIV(a, b) ((a) / (b))
+#endif
 
 #if !defined(PP_HOSTSIM)
 // SM count of the current device, queried once (132 if none answers)

@@ -342,3 +342,82 @@ PP_HD uint8_t pp_mask_overlay(uint8_t img, float mask, int c) {
   const double out = PP_DADD(PP_DMUL(m, fuse), PP_DMUL(PP_DSUB(1.0, m), v));
   return (uint8_t)(int)out;
 }
+
+// ------------------------------------------------------------------------------------------------
+// Optical-flow colour coding: the Middlebury colour wheel of RAFT/utils/flow_viz.py (numpy, one [H,W,2] frame at a
+// time) and RAFT/utils/flow_viz_pt.py (torch, normalised over the whole batch).  Each rule follows the arithmetic the
+// reference executes, one rounding per operation.
+
+// make_colorwheel (flow_viz.py:20-67 = flow_viz_pt.py:73-118): entry k in [0, 55), channel c.  The reference's
+// floor(255 * i / n) is an exact integer quotient here (a non-integral 255 i / n lies >= 1/15 from an integer).
+PP_HD int pp_colorwheel(int k, int c) {
+  int r, g, b;
+  if (k < 15) { r = 255; g = 255 * k / 15; b = 0; }                              // RY
+  else if (k < 21) { r = 255 - 255 * (k - 15) / 6; g = 255; b = 0; }              // YG
+  else if (k < 25) { r = 0; g = 255; b = 255 * (k - 21) / 4; }                    // GC
+  else if (k < 36) { r = 0; g = 255 - 255 * (k - 25) / 11; b = 255; }             // CB
+  else if (k < 49) { r = 255 * (k - 36) / 13; g = 0; b = 255; }                   // BM
+  else { r = 255; g = 0; b = 255 - 255 * (k - 49) / 6; }                          // MR
+  return c == 0 ? r : (c == 1 ? g : b);
+}
+// np.clip(flow, 0, clip_flow) (flow_viz.py:124): minimum(maximum(x, 0), c).  A negative component becomes 0, -0.0 stays
+// -0.0 (it is not below 0) and NaN passes, as numpy does.
+PP_HD float pp_flow_clip(float x, float c) {
+  x = x < 0.0f ? 0.0f : x;
+  return x > c ? c : x;
+}
+// float32 sqrt(u^2 + v^2): rad of flow_viz.py:127 / :88, the norm of flow_viz_pt.py:29 / :55
+PP_HD float pp_flow_rad(float u, float v) { return PP_SQRT(PP_ADD(PP_MUL(u, u), PP_MUL(v, v))); }
+// float32 atan2 rounded once from float64: within half an ulp of the exact angle except for double-rounding ties.
+// numpy's and ATen's float32 atan2 are not correctly rounded (up to 3 ulp off in numpy's AVX-512 path), so a pixel
+// whose colour sits on a rounding boundary may differ by one level (INTEGRATION.md §3).  Signed zeros follow C99:
+// atan2(-0.0, -u) = -pi, atan2(+0.0, -u) = +pi.
+PP_HD float pp_atan2f(float y, float x) { return (float)atan2((double)y, (double)x); }
+// wheel position of a normalised flow vector: (atan2(-v, -u) / pi + 1) / 2 * 54 in float32 (flow_viz.py:89-90,
+// flow_viz_pt.py:56-57; both divide by float32 pi).  k0 is clamped to [0, 54] only for memory safety: a finite input
+// gives fk in [0, 54].
+struct PPWheelPos { float fk; int k0, k1; };
+PP_HD PPWheelPos pp_wheel_pos(float un, float vn) {
+  const float a = PP_DIV(pp_atan2f(-vn, -un), 3.14159274101257324f);
+  PPWheelPos w;
+  w.fk = PP_MUL(PP_DIV(PP_ADD(a, 1.0f), 2.0f), 54.0f);
+  const int k0 = (int)floorf(w.fk);
+  const int k = k0 < 0 ? 0 : (k0 > 54 ? 54 : k0);
+  w.k0 = k;
+  w.k1 = k < 54 ? k + 1 : 0;                                                      // k1[k1 == ncols] = 0
+  return w;
+}
+// numpy variant, one pixel: flow_to_image (flow_viz.py:109-132) + flow_uv_to_colors (:70-106) for float32 input under
+// numpy >= 2 (NEP 50).  den = rad_max + 1e-5 of the (clipped) frame in float32; u, v already clipped.  float32 through
+// fk; f = fk - k0 (float32 - int32) is float64, and so is everything after it: col0/col1, the blend, the rad <= 1
+// lerp (float32 rad widened) and the reachable rad > 1 branch (x 0.75), floor(255 col) cast to uint8.
+PP_HD void pp_flowviz_np(float u, float v, float den, int bgr, uint8_t* rgb) {
+  const float un = PP_DIV(u, den), vn = PP_DIV(v, den);
+  const float rad = pp_flow_rad(un, vn);
+  const PPWheelPos w = pp_wheel_pos(un, vn);
+  const double f = PP_DSUB((double)w.fk, (double)w.k0);
+  for (int c = 0; c < 3; ++c) {
+    const double col0 = PP_DDIV((double)pp_colorwheel(w.k0, c), 255.0);
+    const double col1 = PP_DDIV((double)pp_colorwheel(w.k1, c), 255.0);
+    double col = PP_DADD(PP_DMUL(PP_DSUB(1.0, f), col0), PP_DMUL(f, col1));
+    col = rad <= 1.0f ? PP_DSUB(1.0, PP_DMUL((double)rad, PP_DSUB(1.0, col))) : PP_DMUL(col, 0.75);
+    rgb[bgr ? 2 - c : c] = (uint8_t)(int)floor(PP_DMUL(255.0, col));
+  }
+}
+// torch variant, one pixel: flow_to_image + _normalized_flow_to_image (flow_viz_pt.py:6-70), all float32.  den =
+// max_norm + FLT_EPSILON over the whole batch; ATen's CPU kernel divides (no reciprocal).  No rad > 1 branch: when the
+// largest vector normalises to just above 1, 1 - norm (1 - col) can fall below 0 and floor gives -1, which the
+// float -> uint8 copy wraps to 255 through int32 (x86 ATen); the rule keeps that wrap.
+PP_HD void pp_flowviz_pt(float u, float v, float den, int bgr, uint8_t* rgb) {
+  const float un = PP_DIV(u, den), vn = PP_DIV(v, den);
+  const float norm = pp_flow_rad(un, vn);
+  const PPWheelPos w = pp_wheel_pos(un, vn);
+  const float f = PP_SUB(w.fk, (float)w.k0);
+  for (int c = 0; c < 3; ++c) {
+    const float col0 = PP_DIV((float)pp_colorwheel(w.k0, c), 255.0f);
+    const float col1 = PP_DIV((float)pp_colorwheel(w.k1, c), 255.0f);
+    float col = PP_ADD(PP_MUL(PP_SUB(1.0f, f), col0), PP_MUL(f, col1));
+    col = PP_SUB(1.0f, PP_MUL(norm, PP_SUB(1.0f, col)));
+    rgb[bgr ? 2 - c : c] = (uint8_t)(int)floorf(PP_MUL(255.0f, col));
+  }
+}

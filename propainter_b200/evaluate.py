@@ -85,3 +85,52 @@ def evaluate_clip(pipe, frames_u8, masks_u8, cfg=None, mask_dilation=0, i3d_acti
     if i3d_activations is not None:
         out["i3d"] = (i3d_activations(fr), i3d_activations(comp))
     return out
+
+
+def epe64(flow1, flow2):
+    """calculate_epe (core/metrics.py:12-17) accumulated in float64: mean over pixels of |flow1 - flow2| for [..,2,H,W]"""
+    return ((flow1.double() - flow2.double()) ** 2).sum(-3).sqrt().mean().item()
+
+
+@torch.no_grad()
+def evaluate_flow_clip(pipe, frames_u8, masks_u8, reference_flows=None, cfg=None, mask_dilation=4):
+    """The per-video body of scripts/evaluate_flow_completion.py:88-160: RAFT flows of `frames_u8` ([T,H,W,3] uint8,
+    numpy or tensor), completed by the recurrent flow-completion net under `masks_u8` ([T,H,W], non-zero = hole; made
+    binary and dilated `mask_dilation` times with the 3x3 cross, as TestDataset's cv2.dilate), scored by end-point error.
+
+    As in the script, flow completion runs once over the whole clip (no sub-video chunks), then combine_flow.
+    `reference_flows` (forward, backward), each [1,T-1,2,H,W] or [T-1,2,H,W], are what EPE is measured against; without
+    them the reference is the RAFT flows of the unmasked frames, what scripts/compute_flow.py stores for them.
+    `seconds` is the synchronised wall time of stage 2 alone (:113-137).  Deviation: the script's short-clip branch
+    hard-codes iters=20 where this uses cfg.raft_iter throughout (the default is 20).  EPE is accumulated in float64."""
+    from . import ops
+    from .inference_propainter import InferenceConfig, prepare_masks
+    cfg = cfg or InferenceConfig()
+    dev = pipe.device
+    fr = torch.as_tensor(frames_u8).to(dev)
+    mk = torch.as_tensor(masks_u8).to(dev)
+    fm, _ = prepare_masks(((mk != 0).to(torch.uint8) * 255).contiguous(), mask_dilation, dev)
+    gt =pipe.compute_flows(ops.u8_to_frames(fr).unsqueeze(0), cfg)
+    net = pipe.fix_flow_complete
+    torch.cuda.synchronize(dev)
+    t0 = time.perf_counter()
+    pred, _ = net.forward_bidirect_flow(gt, fm)
+    pred = net.combine_flow(gt, pred, fm)
+    torch.cuda.synchronize(dev)
+    dt = time.perf_counter() - t0
+    ref = gt if reference_flows is None else tuple(torch.as_tensor(r).to(dev).float().reshape(p.shape)
+                                                   for r, p in zip(reference_flows, pred))
+    ef, eb = epe64(ref[0], pred[0]), epe64(ref[1], pred[1])
+    T = fr.shape[0]
+    return {"epe": (ef + eb) / 2, "epe_forward": ef, "epe_backward": eb, "frames": T, "seconds": dt,
+            "seconds_per_frame": dt / T, "pred_flows": pred}
+
+
+def flow_epe_summary(results):
+    """The dataset line of evaluate_flow_completion.py:141-178 over evaluate_flow_clip results: `epe` is the
+    frame-weighted average (total_frame_epe: each direction's EPE counted once per flow), `seconds_per_frame` the mean
+    stage-2 time per frame (time_all)."""
+    flows = [r["frames"] - 1 for r in results]
+    epe = sum(n * (r["epe_forward"] + r["epe_backward"]) for n, r in zip(flows, results)) / (2 * sum(flows))
+    return {"epe": epe, "seconds_per_frame": sum(r["seconds"] for r in results) / sum(r["frames"] for r in results),
+            "videos": len(results)}

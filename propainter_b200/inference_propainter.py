@@ -306,3 +306,28 @@ class ProPainterPipeline:
         dev = self.device
         frames = torch.as_tensor(frames_u8).to(dev, non_blocking=True).contiguous()
         return ops.mask_overlay_u8(frames, masks_dilated.to(dev, non_blocking=True).float().contiguous())
+
+    @torch.no_grad()
+    def flows(self, frames_u8, flow_masks, cfg=None):
+        """Stages 1-2 only (inference_propainter.py:302-368): RAFT flows and the completed flows, with the chunking of
+        __call__ and without image propagation or the generator.  frames_u8 uint8 [T,H,W,3] (host or device), flow_masks
+        float {0,1} [1,T,1,H,W].  Returns (gt_flows, pred_flows), each a (forward, backward) pair of [1,T-1,2,H,W],
+        bit-identical to the stage outputs of __call__(..., return_stages=True)."""
+        cfg = cfg or InferenceConfig()
+        dev = self.device
+        ori = torch.as_tensor(frames_u8).to(dev, non_blocking=True)
+        flow_masks = flow_masks.to(dev, non_blocking=True).float()
+        frames = ops.u8_to_frames(ori).unsqueeze(0)
+        gt = self.compute_flows(frames, cfg)
+        return gt, self.complete_flows(gt, flow_masks, cfg)
+
+    def flow_preview(self, flows, normalize="frame", clip_flow=None, bgr=False):
+        """One direction of a flow pair ([1,T-1,2,H,W] or [T-1,2,H,W] float32) as a colour-coded uint8 video
+        [T-1,H,W,3] on the device; see ops.flow_to_image_u8 for `normalize` ("frame": flow_viz.py, "clip":
+        flow_viz_pt.py), `clip_flow` and `bgr`."""
+        f = flows.to(self.device, non_blocking=True)
+        if f.dim() == 5:
+            if f.shape[0] != 1:
+                raise ValueError(f"flow_preview: expected one clip [1,T-1,2,H,W], got {tuple(flows.shape)}")
+            f = f[0]
+        return ops.flow_to_image_u8(f, normalize, clip_flow, bgr)

@@ -555,6 +555,38 @@ def mask_overlay_u8(frames_u8, masks):
     return out
 
 
+FLOWVIZ_NORMALIZE = {"frame": 0, "clip": 1}       # PP_FLOWVIZ_FRAME / PP_FLOWVIZ_CLIP
+
+
+def flow_to_image_u8(flow, normalize="frame", clip_flow=None, bgr=False):
+    """Middlebury colour coding of planar float32 flow (N,2,H,W) or (2,H,W) on the device -> uint8 (N,H,W,3) or (H,W,3),
+    RGB (BGR with `bgr`).  normalize="frame": RAFT/utils/flow_viz.py::flow_to_image applied to each frame (rad_max per
+    frame, numpy >= 2 arithmetic, the rad > 1 branch); "clip": flow_viz_pt.py::flow_to_image (max_norm over the whole
+    batch).  clip_flow: np.clip(flow, 0, clip_flow) before the radius, as flow_viz.py:123-124 does.  Bytes equal the
+    reference's except where atan2's last-ulp differences move a colour across a rounding boundary (INTEGRATION.md §3).
+    ValueError where flow_viz_pt raises (dtype other than float32, other shapes)."""
+    if flow.dtype != torch.float32:
+        raise ValueError(f"Flow should be of dtype torch.float, got {flow.dtype}.")
+    if normalize not in FLOWVIZ_NORMALIZE:
+        raise ValueError(f"normalize must be 'frame' or 'clip', got {normalize!r}")
+    single = flow.dim() == 3
+    f = flow[None] if single else flow
+    if f.dim() != 4 or f.shape[1] != 2:
+        raise ValueError(f"Input flow should have shape (2, H, W) or (N, 2, H, W), got {tuple(flow.shape)}.")
+    f = f.contiguous()
+    N, _, H, W = f.shape
+    per_frame = int(normalize == "frame")
+    maxima = torch.empty(N if per_frame else 1, dtype=torch.float32, device=f.device)
+    out = torch.empty(N, H, W, 3, dtype=torch.uint8, device=f.device)
+    has_clip, clip = int(clip_flow is not None), ctypes.c_float(0.0 if clip_flow is None else float(clip_flow))
+    L = _lib.lib()
+    check(L.pp_flow_maxrad(_p(f), _p(maxima), N, H, W, per_frame, has_clip, clip, _stream()), "pp_flow_maxrad")
+    check(L.pp_flow_to_image_u8(_p(f), _p(maxima), _p(out, torch.uint8), N, H, W, FLOWVIZ_NORMALIZE[normalize], has_clip,
+                                clip, int(bool(bgr)), _stream()), "pp_flow_to_image_u8")
+    _count(2)
+    return out[0] if single else out
+
+
 # ---------------------------------------------------------------- resizing around the path (tables on the host, passes on the device)
 _TABLES = {}
 
