@@ -49,6 +49,19 @@ int pp_corr_fmap_pyramid(const float* fmap, int D, int frames, int h, int w, flo
  * rule (corr.py:29-50, bilinear_sampler RAFT/utils/utils.py:57-71), so no volume of n_pairs*(h*w)^2 floats is stored. */
 int pp_corr_lookup_otf(const float* fmap, const float* const* pooled, int D, const int* idx1, const int* idx2, int n_pairs,
                        const float* coords, float* out, int h, int w, cudaStream_t stream);
+/* Radius-selectable lookups: radius 4 (the basic model, 324 channels) or 3 (RAFT-small, raft.py:29-33: 4 x 7 x 7 = 196
+ * channels, l*49 + a*7 + b).  Same contracts as pp_corr_lookup / pp_corr_lookup_ldg / pp_corr_lookup_otf with
+ * out [n_pairs*h*w][4*(2*radius+1)^2]; the on-the-fly lookup takes (D, radius) = (256, 4) or (128, 3) and divides by
+ * sqrt(D) rounded to float, as CorrBlock.corr does (corr.py:60).  Any other radius or D: PP_ERR_SHAPE. */
+int pp_corr_lookup_r(const float* const* levels, int radius, const float* coords, float* out, long n_pairs, int h, int w,
+                     cudaStream_t stream);
+int pp_corr_lookup_ldg_r(const float* const* levels, int radius, const float* coords, float* out, long n_pairs, int h, int w,
+                         cudaStream_t stream);
+int pp_corr_lookup_otf_r(const float* fmap, const float* const* pooled, int D, int radius, const int* idx1, const int* idx2,
+                         int n_pairs, const float* coords, float* out, int h, int w, cudaStream_t stream);
+/* upflow8 RAFT/utils/utils.py:80-82 (RAFT-small's upsampling, raft.py:136-137): 8 * bilinear (align_corners=True)
+ * resize to 8h x 8w, bit-exact with ATen's CPU kernel.  flow_lr pixel-major [n][h][w][2] -> out planar [n][2][8h][8w]. */
+int pp_upflow8(const float* flow_lr, float* out, int n, int h, int w, cudaStream_t stream);
 /* RAFT.upsample_flow RAFT/raft.py:73-84.  mask pixel-major [n*h*w][ld_mask>=576] (unscaled conv output,
  * mask_scale = 0.25 from update.py:135); flow_lr [n][h][w][2]; out planar [n][2][8h][8w]. */
 int pp_convex_upsample(const float* mask, int ld_mask, float mask_scale, const float* flow_lr, float* out, int n,
@@ -180,6 +193,10 @@ int pp_gru_update(const float* q, const float* bias, const float* pre, const flo
  * bias != NULL: `mot` is the raw conv output and relu(mot + bias) (RAFT/update.py:96) is applied on the way. */
 int pp_raft_pack_motion(const float* mot, int ld_mot, const float* bias, const float* flow, float* d0, float* d1, int ld,
                         long npix, cudaStream_t stream);
+/* the same for `cmot` motion channels (RAFT-small: 80, update.py:62-77): channels [0,cmot) of `mot` (+ bias, ReLU), then
+ * the 2 flow channels, then zeros up to the slot width roundup4(cmot+2) (<= ld); d0 / d1 16-byte aligned, ld % 4 == 0. */
+int pp_raft_pack_motion_n(const float* mot, int ld_mot, const float* bias, const float* flow, float* d0, float* d1, int ld,
+                          long npix, int cmot, cudaStream_t stream);
 
 /* ---- conv epilogues ------------------------------------------------------------------------- */
 /* out = post(act(x + bias[c]) + res) on pixel-major tensors [n_pix][C] with pixel strides ld_*: replaces the bias add of

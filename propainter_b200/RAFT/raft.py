@@ -1,4 +1,4 @@
-"""RAFT optical flow (basic model) on the H100 hot path.
+"""RAFT optical flow (basic and small models) on the H100 hot path.
 
 Drop-in for the reference's ``RAFT`` (RAFT/raft.py:24-146): same constructor argument, same
 ``forward(image1, image2, iters, flow_init, test_mode)`` result in test mode, same state_dict.
@@ -15,6 +15,11 @@ What differs is the execution plan:
     reference computes them 20x and keeps one, raft.py:135-146)
   * ``flows_bidirectional`` encodes every frame once for both directions (the reference encodes each
     frame up to 4x, flow_comp_raft.py:48-49); per-sample InstanceNorm makes this exactly equivalent
+  * ``args.small`` builds RAFT-small (raft.py:29-33,48-51): SmallEncoders, radius-3 lookups (196 channels) on either
+    plan, the 3x3 ConvGRU with z and r sharing one conv, no mask head -- the flow is upsampled once, after the last
+    iteration, by ``ops.upflow8`` (the reference upsamples every iteration and keeps the last in test mode,
+    raft.py:136-146).  Captured graphs are cached per instance (ParamNet.graphs), so a basic and a small net never
+    share one.
 """
 import torch
 import torch.nn.functional as F
@@ -22,7 +27,7 @@ import torch.nn.functional as F
 from .. import ops
 from .._params import ParamNet
 from ..nn_util import as_nchw, as_pm, cl, conv
-from ..schemas import raft_schema
+from ..schemas import raft_schema, raft_small_schema
 
 
 ALL_PAIRS, ON_THE_FLY = "all_pairs", "on_the_fly"
@@ -30,7 +35,9 @@ ALL_PAIRS, ON_THE_FLY = "all_pairs", "on_the_fly"
 # context / GRU buffers, the 324-channel lookup output, the upsampled flows.  Measured by profiles/raft_mem.py on an
 # H100 80GB HBM3 (700 W power limit): a 2-frame call (2 pairs, 20 iterations) peaked 2,676,002,816 bytes above its
 # inputs at 1280x720, of which 2,200,320,000 are the two pyramids -> 258.1 B per pixel of the 2 frames (257.3 at
-# 1920x1080).  Rounded up.
+# 1920x1080).  Rounded up.  Measured on the basic model; RAFT-small is planned with the same constants: its pyramid has
+# the same size (it depends on the feature grid only) and every other buffer is narrower (128-channel fmap, 196-channel
+# lookup, 96-channel state), so they are upper bounds for it.
 RAFT_WS_BYTES_PER_PX = 260
 # Bytes per input-frame pixel that each pair of an on-the-fly call adds (the same buffers, no pyramid; the pooled
 # feature levels are ~1/3 of fmap): same tool and card, the peak of a 4-frame call (6 pairs) minus that of a
@@ -71,9 +78,12 @@ class RAFT(ParamNet):
     context_dim = 128
 
     def __init__(self, args=None, seed=None):
-        if args is not None and getattr(args, "small", False):
-            raise NotImplementedError("only the basic RAFT model is on ProPainter's path (flow_comp_raft.py:15)")
-        super().__init__(raft_schema(), seed=seed)
+        small = bool(getattr(args, "small", False))
+        super().__init__(raft_small_schema() if small else raft_schema(), seed=seed)
+        self.small = small
+        if small:                                                  # raft.py:29-33
+            self.hidden_dim, self.context_dim = 96, 64
+            args.corr_levels, args.corr_radius = 4, 3
         self.args = args
 
     # ------------------------------------------------------------------ weights
@@ -139,13 +149,42 @@ class RAFT(ParamNet):
                 x = cn(q + ".conv2", q + ".norm2", y, 1, 1, res=x)              # relu(x + relu(norm(conv2(y))))
         return conv(x, self._wb(p + ".conv2"))
 
+    def _encode_small(self, p, x):
+        """SmallEncoder.forward extractor.py:244-267 with BottleneckBlocks (:60-115, 8/16/24 inner channels).  fnet: conv ->
+        InstanceNorm -> ReLU as one pp_instance_norm call on the raw conv output (the bias cancels), the block's
+        `relu(x + y)` fused into the last one.  cnet (norm_fn='none'): conv + bias + ReLU (+ residual + ReLU) through
+        pp_bias_act."""
+        inst = p == "fnet"
+
+        def cn(key, t, stride=1, pad=0, relu=True, res=None):
+            if inst:
+                w, _ = self._wb(key)
+                y = as_pm(F.conv2d(t, w, None, stride=stride, padding=pad))
+                return as_nchw(ops.instance_norm(y, relu=relu, res=None if res is None else as_pm(res),
+                                                 post_relu=res is not None, out=y))
+            return conv(t, self._wb(key), stride, pad, act="relu" if relu else "none", res=res, post_relu=res is not None)
+
+        x = cn(p + ".conv1", x, 2, 3)
+        for li, stride in ((1, 1), (2, 2), (3, 2)):
+            for bi in (0, 1):
+                q = f"{p}.layer{li}.{bi}"
+                s = stride if bi == 0 else 1
+                y = cn(q + ".conv2", cn(q + ".conv1", x), s, 1)
+                if s != 1:
+                    x = cn(q + ".downsample.0", x, s, 0, relu=False)
+                x = cn(q + ".conv3", y, res=x)                               # relu(x + relu(norm(conv3(y))))
+        return conv(x, self._wb(p + ".conv2"))
+
     def encode_frames(self, frames):
-        """frames [n,3,H,W] -> (fmap pixel-major [n, h*w, 256], net [n,128,h,w], inp [n,128,h,w])."""
+        """frames [n,3,H,W] -> (fmap pixel-major [n, h*w, D], net [n,hdim,h,w], inp [n,cdim,h,w]); D = 256 / 128,
+        (hdim, cdim) = (128, 128) / (96, 64) for the basic / small model."""
         x = frames.contiguous(memory_format=torch.channels_last)
-        fmap = as_pm(self._encode("fnet", x).float())
+        enc = self._encode_small if self.small else self._encode
+        fmap = as_pm(enc("fnet", x).float())
         n, h, w, d = fmap.shape
-        c = self._encode("cnet", x)
-        net, inp = torch.tanh(c[:, :128]), torch.relu(c[:, 128:])
+        c = enc("cnet", x)
+        hd = self.hidden_dim
+        net, inp = torch.tanh(c[:, :hd]), torch.relu(c[:, hd:])
         return fmap.view(n, h * w, d), net, inp, (h, w)
 
     # ------------------------------------------------------------------ refinement loop (raft.py:122-146)
@@ -154,6 +193,8 @@ class RAFT(ParamNet):
         return corr_plan(H, W, bool(getattr(self.args, "alternate_corr", False)), device_bytes(device))
 
     def _refine(self, fmap, idx1, idx2, net, inp, hw, iters, plan, flow_init=None):
+        if self.small:
+            return self._refine_small(fmap, idx1, idx2, net, inp, hw, iters, plan, flow_init)
         h, w = hw
         B = idx1.numel()
         dev = fmap.device
@@ -207,6 +248,67 @@ class RAFT(ParamNet):
         mask = conv(conv(net, self._wb(u + "mask.0"), 1, 1, act="relu"), self._wb(u + "mask.2"))
         up = ops.convex_upsample(as_pm(mask), flow_lr.contiguous(), 0.25)
         return as_nchw(flow_lr), up
+
+    def _gru_small(self):
+        """ConvGRU weights (update.py:16-31), input channels [h(96) | inp(64) | motion(80) | flow(2)] (:108-109); z and r
+        share one conv.  As in _gru, the `inp` share of every gate is split off and convolved once per call; the per-
+        iteration convs read [h | motion flow pad(2)] (180 channels, 16-byte rows), the pad weights are zero."""
+        def build():
+            u = "update_block.gru."
+            wzr = torch.cat([self.P[u + "convz.weight"], self.P[u + "convr.weight"]], 0)
+            bzr = torch.cat([self.P[u + "convz.bias"], self.P[u + "convr.bias"]], 0)
+            wq, bq = self.P[u + "convq.weight"], self.P[u + "convq.bias"]
+            dyn = lambda w: cl(torch.cat([w[:, :96], w[:, 160:], w.new_zeros(w.shape[0], 2, *w.shape[2:])], 1))
+            ctx = lambda w: cl(w[:, 96:160])
+            return dyn(wzr), dyn(wq), (ctx(wzr), bzr.contiguous()), (ctx(wq), bq.contiguous())
+        return self.packed("gru_small", build)
+
+    def _refine_small(self, fmap, idx1, idx2, net, inp, hw, iters, plan, flow_init=None):
+        """SmallUpdateBlock refinement (raft.py:122-146, update.py:62-77,99-112) on radius-3 lookups; upflow8 once at the end."""
+        h, w = hw
+        B = idx1.numel()
+        dev = fmap.device
+        R = self.args.corr_radius
+        if plan == ON_THE_FLY:
+            pooled = ops.corr_fmap_pyramid(fmap, h, w)
+            lookup = lambda c, out: ops.corr_lookup_otf_r(fmap, pooled, idx1, idx2, c, R, out)
+        else:
+            levels = ops.corr_alloc(B, h, w, dev)
+            ops.corr_build(fmap, idx1, idx2, levels, h, w)
+            lookup = lambda c, out: ops.corr_lookup_r(levels, c, R, out)
+        ys, xs = torch.meshgrid(torch.arange(h, device=dev), torch.arange(w, device=dev), indexing="ij")
+        c0 = torch.stack([xs, ys], -1).float()[None].expand(B, h, w, 2).contiguous()     # coords_grid (utils.py:74-77)
+        c1 = c0.clone()
+        if flow_init is not None:
+            c1 = c1 + as_pm(flow_init)
+        u = "update_block."
+        corr = torch.empty(B, h, w, 4 * (2 * R + 1) ** 2, device=dev)
+        # HX = [net(96) | motion(80) flow(2) pad(2)] -> z/r gate conv;  RX = [r*net | motion flow pad] -> candidate conv
+        HX = torch.empty(B, h, w, 180, device=dev)
+        RX = torch.empty(B, h, w, 180, device=dev)
+        HX[..., :96] = as_pm(net)
+        gw, qw, zr_ctx, q_ctx = self._gru_small()
+        pre_zr, pre_q = as_pm(conv(inp, zr_ctx, 1, 1)), as_pm(conv(inp, q_ctx, 1, 1))
+        netv, z = HX[..., :96], torch.empty(B, h, w, 96, device=dev)
+        netc = torch.empty(B, h, w, 96, device=dev)             # dense copy of the state for the flow head
+        mot_in = torch.empty(B, h, w, 128, device=dev)          # [cor(96) | flo(32)] without a torch.cat (update.py:74)
+        mw, mb = cl(self.P[u + "encoder.conv.weight"]), self.P[u + "encoder.conv.bias"].contiguous()
+        for _ in range(iters):
+            lookup(c1, corr)
+            flow_pm = c1 - c0
+            flow = as_nchw(flow_pm)
+            conv(as_nchw(corr), self._wb(u + "encoder.convc1"), act="relu", out=as_nchw(mot_in[..., :96]))
+            flo = conv(flow, self._wb(u + "encoder.convf1"), 1, 3, act="relu")
+            conv(flo, self._wb(u + "encoder.convf2"), 1, 1, act="relu", out=as_nchw(mot_in[..., 96:]))
+            mot = F.conv2d(as_nchw(mot_in), mw, None, padding=1)                   # 80 channels, raw
+            ops.raft_pack_motion_n(as_pm(mot), flow_pm, HX[..., 96:], RX[..., 96:], 80, bias=mb)   # + bias + ReLU (update.py:75)
+            ops.gru_gate(as_pm(F.conv2d(as_nchw(HX), gw, None, padding=1)), None, netv, z, RX[..., :96], pre=pre_zr)
+            ops.gru_update(as_pm(F.conv2d(as_nchw(RX), qw, None, padding=1)), None, z, netv, net_copy=netc, pre=pre_q)
+            net = as_nchw(netc)
+            d = conv(conv(net, self._wb(u + "flow_head.conv1"), 1, 1, act="relu"), self._wb(u + "flow_head.conv2"), 1, 1)
+            c1 = c1 + as_pm(d)
+        flow_lr = c1 - c0
+        return as_nchw(flow_lr), ops.upflow8(flow_lr.contiguous())
 
     @torch.no_grad()
     def forward(self, image1, image2, iters=12, flow_init=None, test_mode=True):

@@ -53,6 +53,11 @@ SIGNATURES = {
     "pp_corr_lookup_ldg": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_int, c_int, c_void_p]),
     "pp_corr_fmap_pyramid": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "pp_corr_lookup_otf": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "pp_corr_lookup_r": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_long, c_int, c_int, c_void_p]),
+    "pp_corr_lookup_ldg_r": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_long, c_int, c_int, c_void_p]),
+    "pp_corr_lookup_otf_r": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int,
+                                     c_void_p]),
+    "pp_upflow8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pp_convex_upsample": (c_int, [c_void_p, c_int, c_float, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pp_img_prop_scan_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "pp_img_prop_scan": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_int,
@@ -79,6 +84,7 @@ SIGNATURES = {
     "pp_gru_gate": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_long, c_int, c_void_p]),
     "pp_gru_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_long, c_int, c_void_p]),
     "pp_raft_pack_motion": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_long, c_void_p]),
+    "pp_raft_pack_motion_n": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_long, c_int, c_void_p]),
     "pp_bias_act": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_long, c_int, c_int, c_float, c_int,
                             c_void_p]),
     "pp_bias_act_pre": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_long, c_int, c_int, c_float,

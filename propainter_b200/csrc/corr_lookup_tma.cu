@@ -2,34 +2,47 @@
 //
 // One warp per source pixel.  For each of the 4 pyramid levels the warp's elected lane issues one
 // cp.async.bulk.tensor (TMA, 3-D tiled: x, y, plane) that lands the 16x10 neighbourhood of the lookup
-// centre in shared memory (the box's innermost coordinate is rounded down to a multiple of 4 floats: a
+// centre in shared memory (radius 3: 12x8; the box's innermost coordinate is rounded down to a multiple of 4 floats: a
 // tiled TMA load whose first element is not 16-byte aligned faults with "illegal instruction" -- measured
 // with profiles/probes/tma_probe.cu); out-of-range rows / columns are zero-filled by the TMA unit, which *is*
-// grid_sample's zeros padding, so the inner loop has no bounds logic on loads.  The 81 taps of a level
-// are then bilinear blends of shared-memory values and are written as one contiguous 324-float run.
+// grid_sample's zeros padding, so the inner loop has no bounds logic on loads.  The 81 (radius 3: 49) taps of a level
+// are then bilinear blends of shared-memory values and are written as one contiguous 324-float (196-float) run.
 // Replaces CorrBlock.__call__ (RAFT/corr.py:29-50) + bilinear_sampler (RAFT/utils/utils.py:57-71).
 #include <cuda.h>
 #include "pp_elem.cuh"
 #include "../../include/propainter_b200.h"
 
 #define LK_WARPS 8
-#define LK_BOX 10                       // rows of the staged box: taps b = 0..8 read rows b and b+1
-#define LK_BOXW 16                      // columns: 10 needed + up to 3 because the box must start 16-byte aligned
-#define LK_HALF 4
-#define LK_LVL_FLOATS 192               // 640 B box + pad: level l's box starts 768 B (+0 banks) after level l-1's
+
+// Staging geometry of window radius R (4: the basic model, 3: RAFT-small).  K = 2R+1 taps per axis; taps b = 0..K-1
+// read rows b and b+1, so the box has K+1 rows, and K+1 columns + up to 3 because the box must start 16-byte aligned.
+template <int R> struct LkGeom;
+template <> struct LkGeom<4> {
+  static constexpr int BOX = 10, BOXW = 16;
+  static constexpr int LVL_FLOATS = 192;    // 640 B box + pad: level l's box starts 768 B (+0 banks) after level l-1's
+};
+template <> struct LkGeom<3> {
+  static constexpr int BOX = 8, BOXW = 12;
+  static constexpr int LVL_FLOATS = 96;     // 384 B box: every level's box starts 128-byte aligned
+};
 
 __device__ __forceinline__ uint32_t lk_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+template <int R>
 __device__ __forceinline__ int lk_base(float c, float inv) {
   float v = floorf(c * inv);
   v = fminf(fmaxf(v, -1.0e6f), 1.0e6f);
-  return (int)v - LK_HALF;
+  return (int)v - R;
 }
 
+template <int R>
 __global__ void __launch_bounds__(LK_WARPS * 32) k_corr_lookup_tma(const __grid_constant__ CUtensorMap tm0,
     const __grid_constant__ CUtensorMap tm1, const __grid_constant__ CUtensorMap tm2,
     const __grid_constant__ CUtensorMap tm3, const float* __restrict__ coords, float* __restrict__ out, long npix,
     int h, int w) {
+  constexpr int K = 2 * R + 1, NCH = 4 * K * K;
+  constexpr int LK_BOX = LkGeom<R>::BOX, LK_BOXW = LkGeom<R>::BOXW, LK_LVL_FLOATS = LkGeom<R>::LVL_FLOATS;
+  constexpr int LPP = 32 / K, NPASS = (4 + LPP - 1) / LPP;     // levels per pass of the warp, passes
   __shared__ __align__(128) float patch[LK_WARPS][4][LK_LVL_FLOATS];
   __shared__ __align__(8) unsigned long long bar[LK_WARPS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -39,7 +52,7 @@ __global__ void __launch_bounds__(LK_WARPS * 32) k_corr_lookup_tma(const __grid_
   const uint32_t bar_a = lk_smem(&bar[warp]);
   int bx[4], by[4];
 #pragma unroll
-  for (int l = 0; l < 4; ++l) { bx[l] = lk_base(cx, 1.0f / (float)(1 << l)) & ~3; by[l] = lk_base(cy, 1.0f / (float)(1 << l)); }
+  for (int l = 0; l < 4; ++l) { bx[l] = lk_base<R>(cx, 1.0f / (float)(1 << l)) & ~3; by[l] = lk_base<R>(cy, 1.0f / (float)(1 << l)); }
   if (lane == 0) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a));
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -59,17 +72,19 @@ __global__ void __launch_bounds__(LK_WARPS * 32) k_corr_lookup_tma(const __grid_
                    : "=r"(done) : "r"(bar_a) : "memory");
     if (!done) __trap();
   }
-  float* o = out + pix * 324;
-  // Register-blocked along y: a lane owns one (level, x-tap a) column and slides down the 10 staged rows, so each
-  // shared-memory value is read once per column pair (20 loads for 9 taps instead of 36) and the 9 results of a lane
-  // are 9 consecutive output floats (index l*81 + a*9 + b).  Pass 0: levels 0-2 (27 lanes), pass 1: level 3 (9 lanes).
+  float* o = out + pix * NCH;
+  // Register-blocked along y: a lane owns one (level, x-tap a) column and slides down the K+1 staged rows, so each
+  // shared-memory value is read once per column pair (2(K+1) loads for K taps instead of 4K) and the K results of a lane
+  // are K consecutive output floats (index l*K^2 + a*K + b).  A pass covers LPP levels: R = 4 takes levels 0-2 (27
+  // lanes), then level 3 (9 lanes); R = 3 takes all 4 levels (28 lanes) in one pass.
   // All taps of a level share the fractional part of the centre (integer tap offsets): corners outside the image read
   // the zeros TMA filled in.  (The reference sends every tap through grid_sample's normalise / un-normalise round trip,
   // RAFT/utils/utils.py:60-65, which only adds ~1e-6 px of rounding noise -- dropped, well inside the 1e-4 tolerance.)
 #pragma unroll
-  for (int pass = 0; pass < 2; ++pass) {
-    const int l = pass == 0 ? lane / 9 : 3, a = pass == 0 ? lane - 9 * (lane / 9) : lane;
-    const bool act = pass == 0 ? lane < 27 : lane < 9;
+  for (int pass = 0; pass < NPASS; ++pass) {
+    const int nl = 4 - pass * LPP < LPP ? 4 - pass * LPP : LPP;                 // levels of this pass
+    const int l = nl == 1 ? pass * LPP : pass * LPP + lane / K, a = nl == 1 ? lane : lane - K * (lane / K);
+    const bool act = lane < nl * K;
     if (act) {
       const float inv = 1.0f / (float)(1 << l);
       const float xl = cx * inv, yl = cy * inv;
@@ -78,11 +93,11 @@ __global__ void __launch_bounds__(LK_WARPS * 32) k_corr_lookup_tma(const __grid_
       const float wx0 = sane ? 1.0f - wx1 : 0.f, wy0 = sane ? 1.0f - wy1 : 0.f;
       int bxl = bx[0];
       if (l == 1) bxl = bx[1]; else if (l == 2) bxl = bx[2]; else if (l == 3) bxl = bx[3];
-      const float* q = &patch[warp][l][0] + (lk_base(cx, inv) - bxl) + a;      // row 0 of this lane's column pair
+      const float* q = &patch[warp][l][0] + (lk_base<R>(cx, inv) - bxl) + a;   // row 0 of this lane's column pair
       float top = wx0 * q[0] + wx1 * q[1];
-      float* ol = o + l * 81 + a * 9;
+      float* ol = o + l * (K * K) + a * K;
 #pragma unroll
-      for (int b = 0; b < 9; ++b) {
+      for (int b = 0; b < K; ++b) {
         q += LK_BOXW;
         const float bot = wx0 * q[0] + wx1 * q[1];
         ol[b] = wy0 * top + wy1 * bot;
@@ -105,8 +120,9 @@ static PFN_encodeTiled lk_encoder() {
   return (PFN_encodeTiled)fn;
 }
 
-extern "C" int pp_corr_lookup(const float* const* levels, const float* coords, float* out, long n_pairs, int h, int w,
-                              cudaStream_t stream) {
+template <int R>
+static int corr_lookup_tma(const float* const* levels, const float* coords, float* out, long n_pairs, int h, int w,
+                           cudaStream_t stream) {
   if ((h >> 3) < 2 || (w >> 3) < 2) return PP_ERR_SHAPE;
   const long npix = n_pairs * h * w;
   if (npix > 0x7fffffffL) return PP_ERR_SHAPE;
@@ -118,7 +134,7 @@ extern "C" int pp_corr_lookup(const float* const* levels, const float* coords, f
     const int ld = pp_corr_ld(wl);
     cuuint64_t dims[3] = {(cuuint64_t)ld, (cuuint64_t)hl, (cuuint64_t)npix};
     cuuint64_t strides[2] = {(cuuint64_t)ld * 4, (cuuint64_t)hl * ld * 4};
-    cuuint32_t box[3] = {LK_BOXW, LK_BOX, 1};
+    cuuint32_t box[3] = {LkGeom<R>::BOXW, LkGeom<R>::BOX, 1};
     cuuint32_t estr[3] = {1, 1, 1};
     if (((uintptr_t)levels[l] & 15) != 0) return PP_ERR_ALIGN;
     CUresult r = enc(&tm[l], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)levels[l], dims, strides, box, estr,
@@ -127,8 +143,20 @@ extern "C" int pp_corr_lookup(const float* const* levels, const float* coords, f
     if (r != CUDA_SUCCESS) return PP_ERR_LAUNCH;
     hl >>= 1; wl >>= 1;
   }
-  k_corr_lookup_tma<<<(int)((npix + LK_WARPS - 1) / LK_WARPS), LK_WARPS * 32, 0, stream>>>(tm[0], tm[1], tm[2], tm[3],
-                                                                                           coords, out, npix, h, w);
+  k_corr_lookup_tma<R><<<(int)((npix + LK_WARPS - 1) / LK_WARPS), LK_WARPS * 32, 0, stream>>>(tm[0], tm[1], tm[2], tm[3],
+                                                                                              coords, out, npix, h, w);
   if (cudaPeekAtLastError() != cudaSuccess) return PP_ERR_LAUNCH;
   return PP_OK;
+}
+
+extern "C" int pp_corr_lookup(const float* const* levels, const float* coords, float* out, long n_pairs, int h, int w,
+                              cudaStream_t stream) {
+  return corr_lookup_tma<4>(levels, coords, out, n_pairs, h, w, stream);
+}
+
+extern "C" int pp_corr_lookup_r(const float* const* levels, int radius, const float* coords, float* out, long n_pairs, int h,
+                                int w, cudaStream_t stream) {
+  if (radius == 4) return corr_lookup_tma<4>(levels, coords, out, n_pairs, h, w, stream);
+  if (radius == 3) return corr_lookup_tma<3>(levels, coords, out, n_pairs, h, w, stream);
+  return PP_ERR_SHAPE;
 }

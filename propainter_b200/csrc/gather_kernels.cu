@@ -199,38 +199,53 @@ extern "C" int pp_corr_pool_pyramid(float* const* levels, long planes, int h, in
 
 struct PPLevels { const float* p[4]; };
 
-// One warp per source pixel: 4 levels x 81 taps; each lane walks taps lane, lane+32, ... so that the
-// 324 results of a pixel are written as one contiguous 1296-byte run (pixel-major output feeds the
-// 1x1 motion-encoder conv directly).  The per-pixel planes (<= 6.7 KB + 1.7 + 0.4 + 0.1) stay in L1.
+// One warp per source pixel: 4 levels x K^2 taps (K = 2R+1: 81 for radius 4, 49 for radius 3); each lane walks taps
+// lane, lane+32, ... so that the 4K^2 results of a pixel are written as one contiguous run (pixel-major output feeds
+// the 1x1 motion-encoder conv directly).  The per-pixel planes (<= 6.7 KB + 1.7 + 0.4 + 0.1) stay in L1.
+template <int R>
 __global__ void __launch_bounds__(256) k_corr_lookup(PPLevels lv, const float* __restrict__ coords,
                                                      float* __restrict__ out, long npix, int h, int w) {
+  constexpr int K = 2 * R + 1;
   const int lane = threadIdx.x & 31;
   const long pix = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (pix >= npix) return;
   const float cx = coords[2 * pix], cy = coords[2 * pix + 1];
-  float* o = out + pix * 324;
+  float* o = out + pix * (4 * K * K);
   int hl = h, wl = w;
 #pragma unroll
   for (int l = 0; l < 4; ++l) {
     const int ld = pp_corr_ld(wl);
     const float* plane = lv.p[l] + pix * (long)hl * ld;
-    for (int tap = lane; tap < 81; tap += 32)
-      o[l * 81 + tap] = pp_corr_tap(plane, hl, wl, ld, cx, cy, l, tap / 9, tap % 9);
+    for (int tap = lane; tap < K * K; tap += 32)
+      o[l * (K * K) + tap] = pp_corr_tap_r<R>(plane, hl, wl, ld, cx, cy, l, tap / K, tap % K);
     hl >>= 1; wl >>= 1;
   }
+}
+
+template <int R>
+static int corr_lookup_ldg(const float* const* levels, const float* coords, float* out, long n_pairs, int h, int w,
+                           cudaStream_t stream) {
+  if ((h >> 3) < 2 || (w >> 3) < 2) return PP_ERR_SHAPE;
+  PPLevels lv;
+  for (int l = 0; l < 4; ++l) lv.p[l] = levels[l];
+  const long npix = n_pairs * h * w;
+  k_corr_lookup<R><<<pp_blocks(npix, 8), 256, 0, stream>>>(lv, coords, out, npix, h, w);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
 }
 
 // Plain-load variant of the lookup (kept as the measured baseline of the TMA-staged kernel in
 // corr_lookup_tma.cu; same contract as pp_corr_lookup)
 extern "C" int pp_corr_lookup_ldg(const float* const* levels, const float* coords, float* out, long n_pairs, int h,
                               int w, cudaStream_t stream) {
-  if ((h >> 3) < 2 || (w >> 3) < 2) return PP_ERR_SHAPE;
-  PPLevels lv;
-  for (int l = 0; l < 4; ++l) lv.p[l] = levels[l];
-  const long npix = n_pairs * h * w;
-  k_corr_lookup<<<pp_blocks(npix, 8), 256, 0, stream>>>(lv, coords, out, npix, h, w);
-  PP_LAUNCH_CHECK();
-  return PP_OK;
+  return corr_lookup_ldg<4>(levels, coords, out, n_pairs, h, w, stream);
+}
+// the same with window radius 3 or 4 (pp_corr_lookup_r's contract)
+extern "C" int pp_corr_lookup_ldg_r(const float* const* levels, int radius, const float* coords, float* out, long n_pairs,
+                                    int h, int w, cudaStream_t stream) {
+  if (radius == 4) return corr_lookup_ldg<4>(levels, coords, out, n_pairs, h, w, stream);
+  if (radius == 3) return corr_lookup_ldg<3>(levels, coords, out, n_pairs, h, w, stream);
+  return PP_ERR_SHAPE;
 }
 
 __global__ void __launch_bounds__(256) k_convex_up(const float* __restrict__ mask, int ld_mask, float mask_scale,
@@ -655,6 +670,67 @@ extern "C" int pp_raft_pack_motion(const float* mot, int ld_mot, const float* bi
                                    int ld, long npix, cudaStream_t stream) {
   if (ld % 4 || ld_mot % 4 || ((uintptr_t)bias & 15)) return PP_ERR_ALIGN;
   k_raft_pack_motion<<<pp_blocks(npix * 32, 256), 256, 0, stream>>>(mot, ld_mot, bias, flow, d0, d1, ld, npix);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+
+// the same for a motion conv of any width (RAFT-small: SmallMotionEncoder.conv, 80 channels, update.py:62-77): channels
+// [0,cmot) of `mot` (+ bias, ReLU) and the 2 flow channels fill [0, cmot+2) of the slot, zeros its pad up to
+// roundup4(cmot+2).  Scalar reads: `mot` / `bias` need only cmot channels.
+__global__ void __launch_bounds__(256) k_raft_pack_motion_n(const float* __restrict__ mot, int ld_mot, const float* __restrict__ bias,
+    const float* __restrict__ flow, float* __restrict__ d0, float* __restrict__ d1, int ld, long npix, int cmot) {
+  const int s4 = (cmot + 5) >> 2;                                 // float4 per slot row
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= npix * s4) return;
+  const long pix = i / s4; const int c = (int)(i - pix * s4) * 4;
+  float v[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int e = c + k;
+    float x = 0.f;
+    if (e < cmot) {
+      x = mot[pix * ld_mot + e];
+      if (bias != nullptr) x = fmaxf(x + bias[e], 0.f);
+    } else if (e < cmot + 2) {
+      x = flow[2 * pix + (e - cmot)];
+    }
+    v[k] = x;
+  }
+  const float4 o = make_float4(v[0], v[1], v[2], v[3]);
+  *reinterpret_cast<float4*>(d0 + pix * ld + c) = o;
+  *reinterpret_cast<float4*>(d1 + pix * ld + c) = o;
+}
+extern "C" int pp_raft_pack_motion_n(const float* mot, int ld_mot, const float* bias, const float* flow, float* d0, float* d1,
+                                     int ld, long npix, int cmot, cudaStream_t stream) {
+  if (cmot < 1 || ld_mot < cmot || ld < ((cmot + 5) & ~3) || npix < 0) return PP_ERR_SHAPE;
+  if (ld % 4 || ((uintptr_t)d0 & 15) || ((uintptr_t)d1 & 15)) return PP_ERR_ALIGN;
+  if (npix == 0) return PP_OK;
+  k_raft_pack_motion_n<<<pp_blocks(npix * ((cmot + 5) >> 2), 256), 256, 0, stream>>>(mot, ld_mot, bias, flow, d0, d1, ld, npix, cmot);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+
+// upflow8 of RAFT-small (raft.py:136-137, RAFT/utils/utils.py:80-82): one thread per output pixel, both flow channels.
+// flow_lr pixel-major [n][h][w][2] -> out planar [n][2][8h][8w], the rule of pp_upflow8_coord / pp_upflow8_blend.
+__global__ void __launch_bounds__(256) k_upflow8(const float* __restrict__ flow_lr, float* __restrict__ out, int n, int h, int w) {
+  const long H = 8L * h, W = 8L * w;
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;     // over n*H*W
+  if (i >= (long)n * H * W) return;
+  const long b = i / (H * W), r = i - b * H * W;
+  const int y = (int)(r / W), x = (int)(r - (long)y * W);
+  const PPLin uy = pp_upflow8_coord(y, h), ux = pp_upflow8_coord(x, w);
+  const float2* f = reinterpret_cast<const float2*>(flow_lr) + b * h * w;
+  const float2 v00 = f[(long)uy.i0 * w + ux.i0], v01 = f[(long)uy.i0 * w + ux.i1];
+  const float2 v10 = f[(long)uy.i1 * w + ux.i0], v11 = f[(long)uy.i1 * w + ux.i1];
+  float* o = out + b * 2 * H * W + r;
+  o[0] = pp_upflow8_blend(v00.x, v01.x, v10.x, v11.x, uy, ux);
+  o[H * W] = pp_upflow8_blend(v00.y, v01.y, v10.y, v11.y, uy, ux);
+}
+extern "C" int pp_upflow8(const float* flow_lr, float* out, int n, int h, int w, cudaStream_t stream) {
+  if (n < 1 || h < 1 || w < 1) return PP_ERR_SHAPE;
+  if ((uintptr_t)flow_lr & 7) return PP_ERR_ALIGN;
+  if ((long)n * 64 * h * w / 256 >= 0x7fffffffL) return PP_ERR_SHAPE;
+  k_upflow8<<<pp_blocks((long)n * 64 * h * w, 256), 256, 0, stream>>>(flow_lr, out, n, h, w);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }

@@ -62,6 +62,13 @@ static inline float4 make_float4(float a, float b, float c, float d) { float4 r 
 #define PP_DDIV(a, b) ((a) / (b))
 #endif
 
+// one fused multiply-add, rounded once (where the restated library kernel is compiled with FMA contraction)
+#if defined(__CUDA_ARCH__)
+#define PP_FMA(a, b, c) __fmaf_rn((a), (b), (c))
+#else
+#define PP_FMA(a, b, c) fmaf((a), (b), (c))
+#endif
+
 #if !defined(PP_HOSTSIM)
 // SM count of the current device, queried once (132 if none answers)
 static inline int pp_num_sms() {

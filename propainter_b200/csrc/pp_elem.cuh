@@ -189,39 +189,77 @@ PP_HD float pp_pool4(const float* src, int ld, int y, int x) {
   float s = PP_ADD(PP_ADD(PP_ADD(p[0], p[1]), p[ld]), p[ld + 1]);
   return PP_DIV(s, 4.0f);
 }
-// RAFT/corr.py:29-50: output channel l*81 + a*9 + b samples level l at (cx/2^l + (a-4), cy/2^l + (b-4));
+// RAFT/corr.py:29-50 with radius R (4: the basic model, 3: RAFT-small, raft.py:29-33): output channel
+// l*K^2 + a*K + b (K = 2R+1) samples level l at (cx/2^l + (a-R), cy/2^l + (b-R));
 // note the first window axis moves x (reference quirk: delta = stack(meshgrid(dy,dx)) added to (x,y)).
-PP_HD float pp_corr_tap(const float* plane, int Hl, int Wl, int ld, float cx, float cy, int lvl, int a, int b) {
+template <int R>
+PP_HD float pp_corr_tap_r(const float* plane, int Hl, int Wl, int ld, float cx, float cy, int lvl, int a, int b) {
   float s = (float)(1 << lvl);
-  float x = PP_ADD(PP_DIV(cx, s), (float)(a - 4));
-  float y = PP_ADD(PP_DIV(cy, s), (float)(b - 4));
+  float x = PP_ADD(PP_DIV(cx, s), (float)(a - R));
+  float y = PP_ADD(PP_DIV(cy, s), (float)(b - R));
   PPTaps t = pp_taps(pp_raft_coord(x, Wl), pp_raft_coord(y, Hl), Hl, Wl);
   return pp_tap_plane(plane, ld, t);
 }
-// AlternateCorrBlock (RAFT/corr.py:83-111) without a stored plane: level `lvl` is sampled from a 10x10 tile of dot
-// products, tile[j*10 + i] = f1 . f2_l[ty0 + j][tx0 + i] / sqrt(D) (zero outside the level), whose origin is the
-// floored level centre minus the window radius.  Far-away or non-finite centres get a tile wholly outside the level.
-PP_HD int pp_corr_tile_origin(float c, int lvl) {
+PP_HD float pp_corr_tap(const float* plane, int Hl, int Wl, int ld, float cx, float cy, int lvl, int a, int b) {
+  return pp_corr_tap_r<4>(plane, Hl, Wl, ld, cx, cy, lvl, a, b);
+}
+// AlternateCorrBlock (RAFT/corr.py:83-111) without a stored plane: level `lvl` is sampled from a T x T tile of dot
+// products (T = 2R+2), tile[j*T + i] = f1 . f2_l[ty0 + j][tx0 + i] / sqrt(D) (zero outside the level), whose origin is
+// the floored level centre minus the window radius.  Far-away or non-finite centres get a tile wholly outside the level.
+template <int R>
+PP_HD int pp_corr_tile_origin_r(float c, int lvl) {
   float v = floorf(PP_DIV(c, (float)(1 << lvl)));
   v = fminf(fmaxf(v, -1.0e6f), 1.0e6f);
-  return (int)v - 4;
+  return (int)v - R;
 }
-// Tap (a, b) of level `lvl` from that tile by the rule of pp_corr_tap.  The grid_sample coordinate round trip can move
+PP_HD int pp_corr_tile_origin(float c, int lvl) { return pp_corr_tile_origin_r<4>(c, lvl); }
+// Tap (a, b) of level `lvl` from that tile by the rule of pp_corr_tap_r.  The grid_sample coordinate round trip can move
 // a corner by one step at an integer boundary; a corner that lands off the tile then weighs 0 or a few ulp and is dropped.
-PP_HD float pp_corr_tap_tile(const float* tile, int tx0, int ty0, int Hl, int Wl, float cx, float cy, int lvl, int a, int b) {
+template <int R>
+PP_HD float pp_corr_tap_tile_r(const float* tile, int tx0, int ty0, int Hl, int Wl, float cx, float cy, int lvl, int a, int b) {
+  constexpr int T = 2 * R + 2;
   float s = (float)(1 << lvl);
-  float x = PP_ADD(PP_DIV(cx, s), (float)(a - 4));
-  float y = PP_ADD(PP_DIV(cy, s), (float)(b - 4));
+  float x = PP_ADD(PP_DIV(cx, s), (float)(a - R));
+  float y = PP_ADD(PP_DIV(cy, s), (float)(b - R));
   PPTaps t = pp_taps(pp_raft_coord(x, Wl), pp_raft_coord(y, Hl), Hl, Wl);
   if (!t.any) return 0.f;
   const int i = t.x0 - tx0, j = t.y0 - ty0;
-  const bool i0 = i >= 0 && i < 10, i1 = i >= -1 && i < 9, j0 = j >= 0 && j < 10, j1 = j >= -1 && j < 9;
+  const bool i0 = i >= 0 && i < T, i1 = i >= -1 && i < T - 1, j0 = j >= 0 && j < T, j1 = j >= -1 && j < T - 1;
   float acc = 0.f;
-  if (t.w00 != 0.f && j0 && i0) acc += tile[j * 10 + i] * t.w00;
-  if (t.w01 != 0.f && j0 && i1) acc += tile[j * 10 + i + 1] * t.w01;
-  if (t.w10 != 0.f && j1 && i0) acc += tile[(j + 1) * 10 + i] * t.w10;
-  if (t.w11 != 0.f && j1 && i1) acc += tile[(j + 1) * 10 + i + 1] * t.w11;
+  if (t.w00 != 0.f && j0 && i0) acc += tile[j * T + i] * t.w00;
+  if (t.w01 != 0.f && j0 && i1) acc += tile[j * T + i + 1] * t.w01;
+  if (t.w10 != 0.f && j1 && i0) acc += tile[(j + 1) * T + i] * t.w10;
+  if (t.w11 != 0.f && j1 && i1) acc += tile[(j + 1) * T + i + 1] * t.w11;
   return acc;
+}
+PP_HD float pp_corr_tap_tile(const float* tile, int tx0, int ty0, int Hl, int Wl, float cx, float cy, int lvl, int a, int b) {
+  return pp_corr_tap_tile_r<4>(tile, tx0, ty0, Hl, Wl, cx, cy, lvl, a, b);
+}
+
+// upflow8 (RAFT/utils/utils.py:80-82, RAFT-small's upsampling, raft.py:136-137): 8 * F.interpolate(flow, (8h, 8w),
+// bilinear, align_corners=True), restated from ATen's CPU upsample_bilinear2d: scale = float(in-1) / (out-1),
+// src = scale * dst, i0 = min(floor(src), in-1), l1 = clamp(src - i0, 0, 1), i1 = i0 + (i0 < in-1), l0 = 1 - l1.
+// ATen's x86 build (the AVX2 / AVX-512 copies of the kernel are compiled with FMA) contracts each `t0*w0 + t1*w1` of the
+// separable blend into fma(t0, w0, t1*w1): row values fma(v00, lx0, v01*lx1), then fma(row0, ly0, row1*ly1), then * 8.
+// The rule does exactly that, with explicit roundings; it equals ATen bit for bit on every grid RAFT produces
+// (h, w >= 16; measured with torch 2.11 on x86).  Plain mul-add (no FMA) differs by up to 1 ulp on ~20% of pixels.
+struct PPLin { int i0, i1; float l0, l1; };
+PP_HD PPLin pp_upflow8_coord(int dst, int in) {
+  const int out = 8 * in;
+  const float scale = out > 1 ? PP_DIV((float)(in - 1), (float)(out - 1)) : 0.0f;
+  const float src = PP_MUL(scale, (float)dst);
+  PPLin u;
+  u.i0 = (int)floorf(src);
+  if (u.i0 > in - 1) u.i0 = in - 1;
+  u.l1 = fminf(fmaxf(PP_SUB(src, (float)u.i0), 0.0f), 1.0f);
+  u.i1 = u.i0 + (u.i0 < in - 1 ? 1 : 0);
+  u.l0 = PP_SUB(1.0f, u.l1);
+  return u;
+}
+PP_HD float pp_upflow8_blend(float v00, float v01, float v10, float v11, const PPLin& uy, const PPLin& ux) {
+  const float t0 = PP_FMA(v00, ux.l0, PP_MUL(v01, ux.l1));
+  const float t1 = PP_FMA(v10, ux.l0, PP_MUL(v11, ux.l1));
+  return PP_MUL(8.0f, PP_FMA(t0, uy.l0, PP_MUL(t1, uy.l1)));
 }
 
 // RAFT/raft.py:73-84: convex 8x upsampling of one low-res pixel's (i,j) sub-pixel.

@@ -118,6 +118,42 @@ def corr_lookup_otf(fmap, pooled, idx1, idx2, coords, out=None):
     return out
 
 
+def corr_lookup_r(levels, coords, radius, out=None, tma=True):
+    """corr_lookup with window radius 3 (RAFT-small) or 4: coords [B,h,w,2] -> [B,h,w,4*(2*radius+1)**2]."""
+    B, h, w, _ = coords.shape
+    if out is None:
+        out = torch.empty(B, h, w, 4 * (2 * radius + 1) ** 2, device=coords.device, dtype=torch.float32)
+    fn = _lib.lib().pp_corr_lookup_r if tma else _lib.lib().pp_corr_lookup_ldg_r
+    check(fn(_level_array(levels), radius, _p(_dense(coords)), _p(_dense(out)), B, h, w, _stream()), "pp_corr_lookup_r")
+    _count(1)
+    return out
+
+
+def corr_lookup_otf_r(fmap, pooled, idx1, idx2, coords, radius, out=None):
+    """corr_lookup_otf with (D, radius) = (256, 4) or (128, 3): fmap [frames, h*w, D] -> [B,h,w,4*(2*radius+1)**2]."""
+    B, h, w, _ = coords.shape
+    if idx1.numel() != B or idx2.numel() != B:
+        raise RuntimeError("corr_lookup_otf_r: one (idx1, idx2) entry per coords batch row")
+    if out is None:
+        out = torch.empty(B, h, w, 4 * (2 * radius + 1) ** 2, device=coords.device, dtype=torch.float32)
+    levels = (ctypes.c_void_p * 3)(*[_p(_dense(p)).value for p in pooled])
+    check(_lib.lib().pp_corr_lookup_otf_r(_p(_dense(fmap)), levels, fmap.shape[-1], radius, _p(idx1, torch.int32),
+                                          _p(idx2, torch.int32), B, _p(_dense(coords)), _p(_dense(out)), h, w, _stream()),
+          "pp_corr_lookup_otf_r")
+    _count(1)
+    return out
+
+
+def upflow8(flow_lr):
+    """RAFT-small's upflow8 (RAFT/utils/utils.py:80-82): flow_lr pixel-major [n,h,w,2] -> planar [n,2,8h,8w], bit-exact
+    with 8 * F.interpolate(flow, (8h, 8w), mode="bilinear", align_corners=True) on the CPU."""
+    n, h, w, _ = flow_lr.shape
+    out = torch.empty(n, 2, 8 * h, 8 * w, device=flow_lr.device, dtype=torch.float32)
+    check(_lib.lib().pp_upflow8(_p(_dense(flow_lr)), _p(out), n, h, w, _stream()), "pp_upflow8")
+    _count(1)
+    return out
+
+
 def convex_upsample(mask_pm, flow_lr, mask_scale=0.25):
     """mask_pm [n,h,w,576] pixel-major, flow_lr [n,h,w,2] -> planar [n,2,8h,8w]."""
     n, h, w, _ = flow_lr.shape
@@ -412,6 +448,21 @@ def raft_pack_motion(mot_pm, flow_pm, d0_view, d1_view, bias=None):
         raise RuntimeError("HX / RX must share the pixel stride")
     check(_lib.lib().pp_raft_pack_motion(mp, ldm, _p(bias), _p(_dense(flow_pm)), p0, p1, ld0, flow_pm.numel() // 2, _stream()),
           "pp_raft_pack_motion")
+    _count(1)
+
+
+def raft_pack_motion_n(mot_pm, flow_pm, d0_view, d1_view, cmot, bias=None):
+    """raft_pack_motion for `cmot` motion channels: channels [0,cmot) of mot_pm (+ bias, ReLU), the 2 flow channels, zeros
+    up to roundup4(cmot+2) -> that many channels of the slot views d0_view / d1_view (of HX and RX)."""
+    mp, ldm = _pm(mot_pm)
+    p0, ld0 = _pm(d0_view)
+    p1, ld1 = _pm(d1_view)
+    if ld0 != ld1:
+        raise RuntimeError("HX / RX must share the pixel stride")
+    if mot_pm.shape[-1] < cmot or d0_view.shape[-1] < ((cmot + 5) & ~3) or (bias is not None and bias.numel() < cmot):
+        raise RuntimeError("raft_pack_motion_n: channel counts too small for cmot")
+    check(_lib.lib().pp_raft_pack_motion_n(mp, ldm, _p(bias), _p(_dense(flow_pm)), p0, p1, ld0, flow_pm.numel() // 2, cmot,
+                                           _stream()), "pp_raft_pack_motion_n")
     _count(1)
 
 

@@ -5,7 +5,8 @@ RFC :  model/recurrent_flow_completion.py:9-28,46-65,148-160,172-190,203-264
 GEN :  model/propainter.py:34-54,72-101,193-216,235-304; model/modules/sparse_transformer.py:7-17,
        34-47,64-72,117-153,284-292,321-329
 The golden manifest ``tests/golden/state_dict_manifest.json`` (dumped from the reference modules in
-the authoring container) pins these in the CPU test-suite.
+the authoring container) pins these in the CPU test-suite; ``tests/golden/state_dict_manifest_raft_small.json`` pins
+``raft_small_schema``.
 """
 import torch
 
@@ -48,6 +49,37 @@ def raft_schema():
     S.conv(u + "flow_head.conv2", 256, 2, 3, gain=0.05)   # keeps random-init flow within a few px
     S.conv(u + "mask.0", 128, 256, 3, gain=1.4)
     S.conv(u + "mask.2", 256, 576, 1)
+    return S
+
+
+def raft_small_schema():
+    """RAFT(args.small=True): RAFT/raft.py:29-33,48-51, SmallEncoder RAFT/extractor.py:195-267 with BottleneckBlock :60-115,
+    SmallUpdateBlock RAFT/update.py:16-31,62-77,99-112.  No norm parameters: fnet's InstanceNorm2d has no affine and cnet
+    uses norm_fn='none' (nn.Sequential()), so a strided block's downsample is Sequential(conv, Sequential()) -> key
+    `.downsample.0` only."""
+    S = Schema()
+    for enc, out in (("fnet", 128), ("cnet", 160)):
+        S.conv(f"{enc}.conv1", 3, 32, 7, gain=1.4)
+        cin = 32
+        for li, dim, stride in ((1, 32, 1), (2, 64, 2), (3, 96, 2)):
+            for bi in (0, 1):
+                p = f"{enc}.layer{li}.{bi}"
+                S.conv(p + ".conv1", cin, dim // 4, 1, gain=1.4)
+                S.conv(p + ".conv2", dim // 4, dim // 4, 3, gain=1.4)
+                S.conv(p + ".conv3", dim // 4, dim, 1, gain=1.4)
+                if bi == 0 and stride != 1:
+                    S.conv(p + ".downsample.0", cin, dim, 1)
+                cin = dim
+        S.conv(f"{enc}.conv2", 96, out, 1)
+    u = "update_block."
+    S.conv(u + "encoder.convc1", 196, 96, 1, gain=1.4)
+    S.conv(u + "encoder.convf1", 2, 64, 7, gain=1.4)
+    S.conv(u + "encoder.convf2", 64, 32, 3, gain=1.4)
+    S.conv(u + "encoder.conv", 128, 80, 3, gain=1.4)
+    for gate in "zrq":
+        S.conv(f"{u}gru.conv{gate}", 96 + 146, 96, 3)
+    S.conv(u + "flow_head.conv1", 96, 128, 3, gain=1.4)
+    S.conv(u + "flow_head.conv2", 128, 2, 3, gain=0.05)   # keeps random-init flow within a few px
     return S
 
 
