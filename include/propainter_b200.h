@@ -39,6 +39,12 @@ int pp_corr_lookup(const float* const* levels, const float* coords, float* out, 
 /* same contract, plain global loads instead of TMA staging (baseline for the ncu comparison) */
 int pp_corr_lookup_ldg(const float* const* levels, const float* coords, float* out, long n_pairs, int h, int w,
                        cudaStream_t stream);
+/* pp_corr_lookup / pp_corr_lookup_ldg writing fp16 (each tap blended in fp32, rounded to nearest once) into rows of
+ * ld_out >= 324 halves; channels [324, ld_out) are not written.  The operand of RAFT's half-precision convc1. */
+int pp_corr_lookup_f16(const float* const* levels, const float* coords, void* out, int ld_out, long n_pairs, int h, int w,
+                       cudaStream_t stream);
+int pp_corr_lookup_ldg_f16(const float* const* levels, const float* coords, void* out, int ld_out, long n_pairs, int h, int w,
+                           cudaStream_t stream);
 /* AlternateCorrBlock RAFT/corr.py:83-111 (the memory-free lookup behind args.alternate_corr, raft.py:44-45,106-109):
  * levels 1-3 of the per-frame feature pyramid, 2x2 average pooling with avg_pool2d's floor sizes.  fmap pixel-major
  * [frames][h*w][D] (D % 4 == 0); pooled: host array of 3 device pointers, pooled[l-1] = [frames][(h>>l)*(w>>l)][D]. */
@@ -193,6 +199,16 @@ int pp_gru_update(const float* q, const float* bias, const float* pre, const flo
  * bias != NULL: `mot` is the raw conv output and relu(mot + bias) (RAFT/update.py:96) is applied on the way. */
 int pp_raft_pack_motion(const float* mot, int ld_mot, const float* bias, const float* flow, float* d0, float* d1, int ld,
                         long npix, cudaStream_t stream);
+/* Half-operand variants (fp16 rows 8-byte aligned): the gate / candidate / motion conv outputs (zr, q, mot), rnet, h_img,
+ * net_copy, d0 and d1 are fp16; the recurrent state net, z, bias, pre and flow stay fp32, all arithmetic is fp32 and every
+ * fp16 store rounds to nearest.  pp_gru_update_f16 updates the fp32 state in place and writes its fp16 image to h_img
+ * (the state slice of HX, stride ld_img, nullable) and net_copy (dense, nullable). */
+int pp_gru_gate_f16(const void* zr, const float* bias, const float* pre, const float* net, int ld_net, float* z, void* rnet,
+                    int ld_r, long npix, int C, cudaStream_t stream);
+int pp_gru_update_f16(const void* q, const float* bias, const float* pre, const float* z, float* net, int ld_net, void* h_img,
+                      int ld_img, void* net_copy, long npix, int C, cudaStream_t stream);
+int pp_raft_pack_motion_f16(const void* mot, int ld_mot, const float* bias, const float* flow, void* d0, void* d1, int ld,
+                            long npix, cudaStream_t stream);
 /* the same for `cmot` motion channels (RAFT-small: 80, update.py:62-77): channels [0,cmot) of `mot` (+ bias, ReLU), then
  * the 2 flow channels, then zeros up to the slot width roundup4(cmot+2) (<= ld); d0 / d1 16-byte aligned, ld % 4 == 0. */
 int pp_raft_pack_motion_n(const float* mot, int ld_mot, const float* bias, const float* flow, float* d0, float* d1, int ld,
@@ -211,6 +227,10 @@ int pp_bias_act(const float* x, int ld_x, const float* bias, const float* res, i
  * flow, masks; model/propainter.py:151,171, model/recurrent_flow_completion.py:96-106) is convolved once per scan and added here. */
 int pp_bias_act_pre(const float* x, int ld_x, const float* bias, const float* pre, int ld_pre, const float* res, int ld_res,
                     float* out, int ld_out, long n_pix, int C, int act, float slope, int post_relu, cudaStream_t stream);
+/* pp_bias_act_pre with fp16 x (x_f16 != 0, 8-byte aligned rows) and / or fp16 out (out_f16 != 0, rounded to nearest);
+ * bias, pre, res and the arithmetic stay fp32.  The epilogue of RAFT's half-precision refinement-loop convs. */
+int pp_bias_act_f16(const void* x, int ld_x, int x_f16, const float* bias, const float* pre, int ld_pre, const float* res, int ld_res,
+                    void* out, int ld_out, int out_f16, long n_pix, int C, int act, float slope, int post_relu, cudaStream_t stream);
 
 /* nn.InstanceNorm2d(affine=False, eps) of the RAFT feature encoder (RAFT/extractor.py:18-21,125,168-192) on channels-last
  * maps x [n][HW][C]: out = post(relu?((x - mean) * rstd) + res), statistics per (sample, channel), biased variance.

@@ -24,9 +24,9 @@ What differs is the execution plan:
 import torch
 import torch.nn.functional as F
 
-from .. import ops
+from .. import config, ops
 from .._params import ParamNet
-from ..nn_util import as_nchw, as_pm, cl, conv
+from ..nn_util import as_nchw, as_pm, cl, conv, pad_in_channels
 from ..schemas import raft_schema, raft_small_schema
 
 
@@ -122,6 +122,10 @@ class RAFT(ParamNet):
             return dyn(wzr), dyn(wq), (ctx(wzr), bzr.contiguous()), (ctx(wq), bq.contiguous())
         return self.packed("gru" + tag, build)
 
+    def _half(self, key, fn):
+        """fp16 copy of packed weights `fn()` (biases, 1-D, stay fp32) for the half-operand refinement loop"""
+        return self.packed("f16:" + key, lambda: tuple(t.half() if t.dim() == 4 else t for t in fn()))
+
     # ------------------------------------------------------------------ encoders (extractor.py:168-192)
     def _encode(self, p, x):
         """BasicEncoder.forward extractor.py:168-192.  fnet: conv -> InstanceNorm -> ReLU with the norm, the ReLU and the
@@ -195,6 +199,8 @@ class RAFT(ParamNet):
     def _refine(self, fmap, idx1, idx2, net, inp, hw, iters, plan, flow_init=None):
         if self.small:
             return self._refine_small(fmap, idx1, idx2, net, inp, hw, iters, plan, flow_init)
+        if plan == ALL_PAIRS and fmap.is_cuda and config.half_convs():      # cuDNN convs only: elsewhere there is no TF32
+            return self._refine_half(fmap, idx1, idx2, net, inp, hw, iters, flow_init)
         h, w = hw
         B = idx1.numel()
         dev = fmap.device
@@ -245,6 +251,69 @@ class RAFT(ParamNet):
             d = conv(conv(net, self._wb(u + "flow_head.conv1"), 1, 1, act="relu"), self._wb(u + "flow_head.conv2"), 1, 1)
             c1 = c1 + as_pm(d)
         flow_lr = c1 - c0
+        mask = conv(conv(net, self._wb(u + "mask.0"), 1, 1, act="relu"), self._wb(u + "mask.2"))
+        up = ops.convex_upsample(as_pm(mask), flow_lr.contiguous(), 0.25)
+        return as_nchw(flow_lr), up
+
+    def _refine_half(self, fmap, idx1, idx2, net, inp, hw, iters, flow_init=None):
+        """_refine on the all-pairs plan with half-precision operands (config.HALF_OPERANDS, DESIGN.md §4 "Precision"):
+        the lookup output, the motion features, HX / RX and the inputs of convc1, convc2, convf2, the motion conv, the
+        four SepConvGRU gate convs and flow_head.conv1 are fp16 (rounded to nearest by the producing kernel), the convs
+        accumulate in fp32 and every epilogue computes in fp32.  The recurrent state (`netf`, HX / RX hold its fp16
+        image), the coordinates, the context shares `pre`, convf1 (7x7 on the flow), flow_head.conv2 and the mask head
+        stay fp32."""
+        h, w = hw
+        B = idx1.numel()
+        dev = fmap.device
+        f16 = torch.float16
+        levels = ops.corr_alloc(B, h, w, dev)
+        ops.corr_build(fmap, idx1, idx2, levels, h, w)
+        ys, xs = torch.meshgrid(torch.arange(h, device=dev), torch.arange(w, device=dev), indexing="ij")
+        c0 = torch.stack([xs, ys], -1).float()[None].expand(B, h, w, 2).contiguous()     # coords_grid (utils.py:74-77)
+        c1 = c0.clone()
+        if flow_init is not None:
+            c1 = c1 + as_pm(flow_init)
+        u = "update_block."
+        corr = torch.zeros(B, h, w, 328, device=dev, dtype=f16)   # 324 taps + 4 zero channels: 16-byte pixel rows
+        HX = torch.empty(B, h, w, 256, device=dev, dtype=f16)
+        RX = torch.empty(B, h, w, 256, device=dev, dtype=f16)
+        netf = torch.empty(B, h, w, 128, device=dev)
+        netf.copy_(as_pm(net))
+        HX[..., :128] = netf
+        pre = {}
+        for tag, pad in (("1", (0, 2)), ("2", (2, 0))):
+            _, _, zr_ctx, q_ctx = self._gru(tag)
+            pre[tag] = (as_pm(conv(inp, zr_ctx, 1, pad)), as_pm(conv(inp, q_ctx, 1, pad)))
+        z = torch.empty(B, h, w, 128, device=dev)
+        netc = torch.empty(B, h, w, 128, device=dev, dtype=f16)   # dense fp16 image of the state for flow_head.conv1
+        mot_in = torch.empty(B, h, w, 256, device=dev, dtype=f16)
+        mw, mb = self._half("motion_out", self._motion_out)
+        c1w = self._half("convc1", lambda: (cl(pad_in_channels(self._wb(u + "encoder.convc1")[0], 328)),
+                                            self._wb(u + "encoder.convc1")[1]))
+        wb16 = lambda k: self._half(k, lambda: self._wb(u + k))
+
+        def ep(x, wb, pad, out):
+            """conv (no bias) + bias + ReLU into the pixel-major `out` (fp16 or fp32) through pp_bias_act_f16"""
+            return as_nchw(ops.bias_act(as_pm(F.conv2d(x, wb[0], None, padding=pad)), wb[1], "relu", out=out))
+
+        for _ in range(iters):
+            ops.corr_lookup(levels, c1, corr)
+            flow_pm = c1 - c0
+            cor = ep(as_nchw(corr), c1w, 0, torch.empty(B, h, w, 256, device=dev, dtype=f16))
+            ep(cor, wb16("encoder.convc2"), 1, mot_in[..., :192])
+            flo = ep(as_nchw(flow_pm), self._wb(u + "encoder.convf1"), 3, torch.empty(B, h, w, 128, device=dev, dtype=f16))
+            ep(flo, wb16("encoder.convf2"), 1, mot_in[..., 192:])
+            mot = F.conv2d(as_nchw(mot_in), mw, None, padding=1)                   # 126 real + 2 pad channels, raw
+            ops.raft_pack_motion(as_pm(mot), flow_pm, HX[..., 128:], RX[..., 128:], bias=mb)   # + bias + ReLU (update.py:96)
+            for tag, pad in (("1", (0, 2)), ("2", (2, 0))):
+                gw, qw = self._half("gru" + tag, lambda: self._gru(tag)[:2])
+                ops.gru_gate(as_pm(F.conv2d(as_nchw(HX), gw, None, padding=pad)), None, netf, z, RX[..., :128], pre=pre[tag][0])
+                ops.gru_update(as_pm(F.conv2d(as_nchw(RX), qw, None, padding=pad)), None, z, netf,
+                               net_copy=netc if tag == "2" else None, pre=pre[tag][1], h_img=HX[..., :128])
+            fh = ep(as_nchw(netc), wb16("flow_head.conv1"), 1, torch.empty(B, h, w, 256, device=dev))
+            c1 = c1 + as_pm(conv(fh, self._wb(u + "flow_head.conv2"), 1, 1))
+        flow_lr = c1 - c0
+        net = as_nchw(netf)
         mask = conv(conv(net, self._wb(u + "mask.0"), 1, 1, act="relu"), self._wb(u + "mask.2"))
         up = ops.convex_upsample(as_pm(mask), flow_lr.contiguous(), 0.25)
         return as_nchw(flow_lr), up

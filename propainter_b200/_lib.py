@@ -51,6 +51,8 @@ SIGNATURES = {
     "pp_corr_pool_pyramid": (c_int, [c_void_p, c_long, c_int, c_int, c_void_p]),
     "pp_corr_lookup": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_int, c_int, c_void_p]),
     "pp_corr_lookup_ldg": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_int, c_int, c_void_p]),
+    "pp_corr_lookup_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_long, c_int, c_int, c_void_p]),
+    "pp_corr_lookup_ldg_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_long, c_int, c_int, c_void_p]),
     "pp_corr_fmap_pyramid": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "pp_corr_lookup_otf": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "pp_corr_lookup_r": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_long, c_int, c_int, c_void_p]),
@@ -84,11 +86,17 @@ SIGNATURES = {
     "pp_gru_gate": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_long, c_int, c_void_p]),
     "pp_gru_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_long, c_int, c_void_p]),
     "pp_raft_pack_motion": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_long, c_void_p]),
+    "pp_gru_gate_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_long, c_int, c_void_p]),
+    "pp_gru_update_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_long, c_int,
+                                  c_void_p]),
+    "pp_raft_pack_motion_f16": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_long, c_void_p]),
     "pp_raft_pack_motion_n": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_long, c_int, c_void_p]),
     "pp_bias_act": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_long, c_int, c_int, c_float, c_int,
                             c_void_p]),
     "pp_bias_act_pre": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_long, c_int, c_int, c_float,
                                 c_int, c_void_p]),
+    "pp_bias_act_f16": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_long, c_int,
+                                c_int, c_float, c_int, c_void_p]),
     "pp_pool_depthwise": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "pp_add_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_long, c_int, c_float, c_void_p]),
     "pp_instance_norm_workspace_bytes": (c_size_t, [c_int, c_long, c_int]),

@@ -19,6 +19,12 @@ SCAN_PRIORITY   capture the recurrent propagation scans as high-priority branche
                 Environment: PP_SCAN_PRIORITY=0|1.
 GRAPH_MAX_INPUT_BYTES  stage calls whose inputs exceed this run eagerly instead of as a captured graph (memory: a capture keeps
                 its whole working set alive in a private pool).
+HALF_OPERANDS   RAFT's refinement-loop convs (convc1, convc2, convf2, the motion conv, the four SepConvGRU gate convs,
+                flow_head.conv1) take fp16 operands with fp32 accumulation, on the all-pairs correlation plan.  fp16 has TF32's
+                10 mantissa bits, so this replaces TF32 by the same precision class at twice the tensor rate and half the bytes;
+                it is active only while cuDNN may use TF32 (torch.backends.cudnn.allow_tf32), so a strict-fp32 run stays
+                strict.  The recurrent state, the coordinates and every other conv stay fp32 (DESIGN.md §4 "Precision").
+                Environment: PP_HALF_OPERANDS=0|1.
 AUTOTUNE        time numerically equivalent plans of a step once per shape during warm-up and keep the faster
                 (propainter_b200/autotune.py): grouped conv vs per-group dense convs, conv + pp_bias_act vs cuDNN's fused
                 conv-bias-ReLU.
@@ -35,8 +41,14 @@ FUSED_EPILOGUE = True
 AUTOTUNE = True
 GRAPH_MAX_INPUT_BYTES = 256 << 20      # C2 calls (<= ~170 MB) are graphed; 720p calls run eagerly (80 GB)
 SCAN_PRIORITY = os.environ.get("PP_SCAN_PRIORITY", "1") != "0"
+HALF_OPERANDS = os.environ.get("PP_HALF_OPERANDS", "1") != "0"
 _u = os.environ.get("PP_UMMA_CONV", "auto")
 UMMA_CONV = _u if _u in ("auto", "hybrid", "hoisted") else (_u != "0")
+
+
+def half_convs():
+    """whether RAFT's refinement-loop convs run on fp16 operands now (HALF_OPERANDS where cuDNN may use TF32)"""
+    return bool(HALF_OPERANDS) and torch.backends.cudnn.allow_tf32
 
 
 @contextlib.contextmanager

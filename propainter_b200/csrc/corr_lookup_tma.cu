@@ -35,10 +35,12 @@ __device__ __forceinline__ int lk_base(float c, float inv) {
   return (int)v - R;
 }
 
-template <int R>
+// TO = __half: the taps are blended in fp32 and rounded to nearest once, into rows of ld_out >= 4K^2 halves (the operand
+// of the half-precision convc1); TO = float: ld_out = 4K^2.
+template <int R, typename TO>
 __global__ void __launch_bounds__(LK_WARPS * 32) k_corr_lookup_tma(const __grid_constant__ CUtensorMap tm0,
     const __grid_constant__ CUtensorMap tm1, const __grid_constant__ CUtensorMap tm2,
-    const __grid_constant__ CUtensorMap tm3, const float* __restrict__ coords, float* __restrict__ out, long npix,
+    const __grid_constant__ CUtensorMap tm3, const float* __restrict__ coords, TO* __restrict__ out, int ld_out, long npix,
     int h, int w) {
   constexpr int K = 2 * R + 1, NCH = 4 * K * K;
   constexpr int LK_BOX = LkGeom<R>::BOX, LK_BOXW = LkGeom<R>::BOXW, LK_LVL_FLOATS = LkGeom<R>::LVL_FLOATS;
@@ -72,7 +74,7 @@ __global__ void __launch_bounds__(LK_WARPS * 32) k_corr_lookup_tma(const __grid_
                    : "=r"(done) : "r"(bar_a) : "memory");
     if (!done) __trap();
   }
-  float* o = out + pix * NCH;
+  TO* o = out + pix * ld_out;
   // Register-blocked along y: a lane owns one (level, x-tap a) column and slides down the K+1 staged rows, so each
   // shared-memory value is read once per column pair (2(K+1) loads for K taps instead of 4K) and the K results of a lane
   // are K consecutive output floats (index l*K^2 + a*K + b).  A pass covers LPP levels: R = 4 takes levels 0-2 (27
@@ -95,12 +97,12 @@ __global__ void __launch_bounds__(LK_WARPS * 32) k_corr_lookup_tma(const __grid_
       if (l == 1) bxl = bx[1]; else if (l == 2) bxl = bx[2]; else if (l == 3) bxl = bx[3];
       const float* q = &patch[warp][l][0] + (lk_base<R>(cx, inv) - bxl) + a;   // row 0 of this lane's column pair
       float top = wx0 * q[0] + wx1 * q[1];
-      float* ol = o + l * (K * K) + a * K;
+      TO* ol = o + l * (K * K) + a * K;
 #pragma unroll
       for (int b = 0; b < K; ++b) {
         q += LK_BOXW;
         const float bot = wx0 * q[0] + wx1 * q[1];
-        ol[b] = wy0 * top + wy1 * bot;
+        pp_st1(ol + b, wy0 * top + wy1 * bot);
         top = bot;
       }
     }
@@ -120,8 +122,8 @@ static PFN_encodeTiled lk_encoder() {
   return (PFN_encodeTiled)fn;
 }
 
-template <int R>
-static int corr_lookup_tma(const float* const* levels, const float* coords, float* out, long n_pairs, int h, int w,
+template <int R, typename TO>
+static int corr_lookup_tma(const float* const* levels, const float* coords, TO* out, int ld_out, long n_pairs, int h, int w,
                            cudaStream_t stream) {
   if ((h >> 3) < 2 || (w >> 3) < 2) return PP_ERR_SHAPE;
   const long npix = n_pairs * h * w;
@@ -143,20 +145,26 @@ static int corr_lookup_tma(const float* const* levels, const float* coords, floa
     if (r != CUDA_SUCCESS) return PP_ERR_LAUNCH;
     hl >>= 1; wl >>= 1;
   }
-  k_corr_lookup_tma<R><<<(int)((npix + LK_WARPS - 1) / LK_WARPS), LK_WARPS * 32, 0, stream>>>(tm[0], tm[1], tm[2], tm[3],
-                                                                                              coords, out, npix, h, w);
+  k_corr_lookup_tma<R, TO><<<(int)((npix + LK_WARPS - 1) / LK_WARPS), LK_WARPS * 32, 0, stream>>>(tm[0], tm[1], tm[2], tm[3],
+                                                                                                  coords, out, ld_out, npix, h, w);
   if (cudaPeekAtLastError() != cudaSuccess) return PP_ERR_LAUNCH;
   return PP_OK;
 }
 
 extern "C" int pp_corr_lookup(const float* const* levels, const float* coords, float* out, long n_pairs, int h, int w,
                               cudaStream_t stream) {
-  return corr_lookup_tma<4>(levels, coords, out, n_pairs, h, w, stream);
+  return corr_lookup_tma<4>(levels, coords, out, 324, n_pairs, h, w, stream);
+}
+
+extern "C" int pp_corr_lookup_f16(const float* const* levels, const float* coords, void* out, int ld_out, long n_pairs, int h,
+                                  int w, cudaStream_t stream) {
+  if (ld_out < 324) return PP_ERR_SHAPE;
+  return corr_lookup_tma<4>(levels, coords, (__half*)out, ld_out, n_pairs, h, w, stream);
 }
 
 extern "C" int pp_corr_lookup_r(const float* const* levels, int radius, const float* coords, float* out, long n_pairs, int h,
                                 int w, cudaStream_t stream) {
-  if (radius == 4) return corr_lookup_tma<4>(levels, coords, out, n_pairs, h, w, stream);
-  if (radius == 3) return corr_lookup_tma<3>(levels, coords, out, n_pairs, h, w, stream);
+  if (radius == 4) return corr_lookup_tma<4>(levels, coords, out, 324, n_pairs, h, w, stream);
+  if (radius == 3) return corr_lookup_tma<3>(levels, coords, out, 196, n_pairs, h, w, stream);
   return PP_ERR_SHAPE;
 }

@@ -202,34 +202,34 @@ struct PPLevels { const float* p[4]; };
 // One warp per source pixel: 4 levels x K^2 taps (K = 2R+1: 81 for radius 4, 49 for radius 3); each lane walks taps
 // lane, lane+32, ... so that the 4K^2 results of a pixel are written as one contiguous run (pixel-major output feeds
 // the 1x1 motion-encoder conv directly).  The per-pixel planes (<= 6.7 KB + 1.7 + 0.4 + 0.1) stay in L1.
-template <int R>
+template <int R, typename TO>
 __global__ void __launch_bounds__(256) k_corr_lookup(PPLevels lv, const float* __restrict__ coords,
-                                                     float* __restrict__ out, long npix, int h, int w) {
+                                                     TO* __restrict__ out, int ld_out, long npix, int h, int w) {
   constexpr int K = 2 * R + 1;
   const int lane = threadIdx.x & 31;
   const long pix = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (pix >= npix) return;
   const float cx = coords[2 * pix], cy = coords[2 * pix + 1];
-  float* o = out + pix * (4 * K * K);
+  TO* o = out + pix * ld_out;
   int hl = h, wl = w;
 #pragma unroll
   for (int l = 0; l < 4; ++l) {
     const int ld = pp_corr_ld(wl);
     const float* plane = lv.p[l] + pix * (long)hl * ld;
     for (int tap = lane; tap < K * K; tap += 32)
-      o[l * (K * K) + tap] = pp_corr_tap_r<R>(plane, hl, wl, ld, cx, cy, l, tap / K, tap % K);
+      pp_st1(o + l * (K * K) + tap, pp_corr_tap_r<R>(plane, hl, wl, ld, cx, cy, l, tap / K, tap % K));
     hl >>= 1; wl >>= 1;
   }
 }
 
-template <int R>
-static int corr_lookup_ldg(const float* const* levels, const float* coords, float* out, long n_pairs, int h, int w,
+template <int R, typename TO>
+static int corr_lookup_ldg(const float* const* levels, const float* coords, TO* out, int ld_out, long n_pairs, int h, int w,
                            cudaStream_t stream) {
   if ((h >> 3) < 2 || (w >> 3) < 2) return PP_ERR_SHAPE;
   PPLevels lv;
   for (int l = 0; l < 4; ++l) lv.p[l] = levels[l];
   const long npix = n_pairs * h * w;
-  k_corr_lookup<R><<<pp_blocks(npix, 8), 256, 0, stream>>>(lv, coords, out, npix, h, w);
+  k_corr_lookup<R, TO><<<pp_blocks(npix, 8), 256, 0, stream>>>(lv, coords, out, ld_out, npix, h, w);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }
@@ -238,13 +238,19 @@ static int corr_lookup_ldg(const float* const* levels, const float* coords, floa
 // corr_lookup_tma.cu; same contract as pp_corr_lookup)
 extern "C" int pp_corr_lookup_ldg(const float* const* levels, const float* coords, float* out, long n_pairs, int h,
                               int w, cudaStream_t stream) {
-  return corr_lookup_ldg<4>(levels, coords, out, n_pairs, h, w, stream);
+  return corr_lookup_ldg<4>(levels, coords, out, 324, n_pairs, h, w, stream);
+}
+// fp16 output rows of ld_out >= 324 halves (pp_corr_lookup_f16's contract)
+extern "C" int pp_corr_lookup_ldg_f16(const float* const* levels, const float* coords, void* out, int ld_out, long n_pairs, int h,
+                                      int w, cudaStream_t stream) {
+  if (ld_out < 324) return PP_ERR_SHAPE;
+  return corr_lookup_ldg<4>(levels, coords, (__half*)out, ld_out, n_pairs, h, w, stream);
 }
 // the same with window radius 3 or 4 (pp_corr_lookup_r's contract)
 extern "C" int pp_corr_lookup_ldg_r(const float* const* levels, int radius, const float* coords, float* out, long n_pairs,
                                     int h, int w, cudaStream_t stream) {
-  if (radius == 4) return corr_lookup_ldg<4>(levels, coords, out, n_pairs, h, w, stream);
-  if (radius == 3) return corr_lookup_ldg<3>(levels, coords, out, n_pairs, h, w, stream);
+  if (radius == 4) return corr_lookup_ldg<4>(levels, coords, out, 324, n_pairs, h, w, stream);
+  if (radius == 3) return corr_lookup_ldg<3>(levels, coords, out, 196, n_pairs, h, w, stream);
   return PP_ERR_SHAPE;
 }
 
@@ -392,15 +398,17 @@ extern "C" int pp_ffn_overlap_add(const float* Y, int ldy, float* Z, int ldz, in
 // out = post(act(x + bias[c]) + res) on pixel-major tensors with explicit pixel strides: one pass instead of cuDNN's
 // separate bias add_ kernel, the activation kernel, the residual add and (with a strided `out`) the torch.cat that
 // would place the result into a concat buffer.  act: 0 none, 1 relu, 2 leaky(slope), 3 sigmoid, 4 tanh; bias / res may
-// be NULL; post_relu applies a final ReLU (residual blocks).  out may alias x.
-__global__ void __launch_bounds__(256) k_bias_act(const float* x, int ld_x, const float* __restrict__ bias, const float* res,
-                                                  int ld_res, float* out, int ld_out, long n_pix, int C, int act, float slope,
+// be NULL; post_relu applies a final ReLU (residual blocks).  out may alias x.  TX / TO: fp32 or fp16 rows of x / out
+// (the half-operand convs of RAFT's refinement loop); bias, pre, res and the arithmetic stay fp32.
+template <typename TX, typename TO>
+__global__ void __launch_bounds__(256) k_bias_act(const TX* x, int ld_x, const float* __restrict__ bias, const float* res,
+                                                  int ld_res, TO* out, int ld_out, long n_pix, int C, int act, float slope,
                                                   int post_relu, const float* __restrict__ pre = nullptr, int ld_pre = 0) {
   const int c4n = C >> 2;
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_pix * c4n) return;
   const long pix = i / c4n; const int c = (int)(i - pix * c4n) * 4;
-  const float4 v = *reinterpret_cast<const float4*>(x + pix * ld_x + c);
+  const float4 v = pp_ld4(x + pix * ld_x + c);
   float r[4] = {v.x, v.y, v.z, v.w};
   if (bias != nullptr) {
     const float4 b = *reinterpret_cast<const float4*>(bias + c);
@@ -427,7 +435,7 @@ __global__ void __launch_bounds__(256) k_bias_act(const float* x, int ld_x, cons
 #pragma unroll
     for (int k = 0; k < 4; ++k) r[k] = fmaxf(r[k], 0.f);
   }
-  *reinterpret_cast<float4*>(out + pix * ld_out + c) = make_float4(r[0], r[1], r[2], r[3]);
+  pp_st4(out + pix * ld_out + c, make_float4(r[0], r[1], r[2], r[3]));
 }
 // replaces the bias add of F.conv2d, the following ReLU / LeakyReLU / sigmoid / tanh call, the residual `x + y`
 // (+ ReLU) of the encoder blocks / propagation backbones, and the torch.cat into a concat buffer
@@ -437,8 +445,8 @@ extern "C" int pp_bias_act(const float* x, int ld_x, const float* bias, const fl
   if (((uintptr_t)x & 15) || ((uintptr_t)out & 15) || ((uintptr_t)bias & 15) || ((uintptr_t)res & 15)) return PP_ERR_ALIGN;
   if (ld_x < C || ld_out < C || (res && ld_res < C) || act < 0 || act > 4) return PP_ERR_SHAPE;
   if (n_pix <= 0) return PP_OK;
-  k_bias_act<<<pp_blocks(n_pix * (C / 4), 256), 256, 0, stream>>>(x, ld_x, bias, res, ld_res, out, ld_out, n_pix, C, act, slope,
-                                                                post_relu);
+  k_bias_act<float, float><<<pp_blocks(n_pix * (C / 4), 256), 256, 0, stream>>>(x, ld_x, bias, res, ld_res, out, ld_out, n_pix, C,
+                                                                              act, slope, post_relu);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }
@@ -456,8 +464,35 @@ extern "C" int pp_bias_act_pre(const float* x, int ld_x, const float* bias, cons
     return PP_ERR_ALIGN;
   if (ld_x < C || ld_out < C || ld_pre < C || (res && ld_res < C) || act < 0 || act > 4) return PP_ERR_SHAPE;
   if (n_pix <= 0) return PP_OK;
-  k_bias_act<<<pp_blocks(n_pix * (C / 4), 256), 256, 0, stream>>>(x, ld_x, bias, res, ld_res, out, ld_out, n_pix, C, act, slope,
-                                                                post_relu, pre, ld_pre);
+  k_bias_act<float, float><<<pp_blocks(n_pix * (C / 4), 256), 256, 0, stream>>>(x, ld_x, bias, res, ld_res, out, ld_out, n_pix, C,
+                                                                              act, slope, post_relu, pre, ld_pre);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+
+// pp_bias_act_pre with fp16 x (x_f16) and / or fp16 out (out_f16); fp16 rows 8-byte aligned, fp32 ones 16-byte.
+extern "C" int pp_bias_act_f16(const void* x, int ld_x, int x_f16, const float* bias, const float* pre, int ld_pre, const float* res,
+                               int ld_res, void* out, int ld_out, int out_f16, long n_pix, int C, int act, float slope, int post_relu,
+                               cudaStream_t stream) {
+  if (C % 4 || ld_x % 4 || ld_out % 4 || (pre && ld_pre % 4) || (res && ld_res % 4)) return PP_ERR_ALIGN;
+  if (((uintptr_t)x & (x_f16 ? 7 : 15)) || ((uintptr_t)out & (out_f16 ? 7 : 15)) || ((uintptr_t)bias & 15) || ((uintptr_t)res & 15) ||
+      ((uintptr_t)pre & 15))
+    return PP_ERR_ALIGN;
+  if (ld_x < C || ld_out < C || (pre && ld_pre < C) || (res && ld_res < C) || act < 0 || act > 4) return PP_ERR_SHAPE;
+  if (n_pix <= 0) return PP_OK;
+  const int nb = pp_blocks(n_pix * (C / 4), 256);
+  if (x_f16 && out_f16)
+    k_bias_act<__half, __half><<<nb, 256, 0, stream>>>((const __half*)x, ld_x, bias, res, ld_res, (__half*)out, ld_out, n_pix, C, act,
+                                                       slope, post_relu, pre, ld_pre);
+  else if (x_f16)
+    k_bias_act<__half, float><<<nb, 256, 0, stream>>>((const __half*)x, ld_x, bias, res, ld_res, (float*)out, ld_out, n_pix, C, act,
+                                                      slope, post_relu, pre, ld_pre);
+  else if (out_f16)
+    k_bias_act<float, __half><<<nb, 256, 0, stream>>>((const float*)x, ld_x, bias, res, ld_res, (__half*)out, ld_out, n_pix, C, act,
+                                                      slope, post_relu, pre, ld_pre);
+  else
+    k_bias_act<float, float><<<nb, 256, 0, stream>>>((const float*)x, ld_x, bias, res, ld_res, (float*)out, ld_out, n_pix, C, act,
+                                                     slope, post_relu, pre, ld_pre);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }
@@ -592,14 +627,17 @@ extern "C" int pp_upsample2x_bilinear(const float* src, float* dst, int n, int h
 //   HX = [net | inp | motion | flow]   (input of the z/r gate conv)
 //   RX = [r*net | inp | motion | flow] (input of the candidate conv)
 // so no torch.cat is needed inside the 20-iteration loop.
-__global__ void __launch_bounds__(256) k_gru_gate(const float* __restrict__ zr, const float* __restrict__ bias,
-    const float* __restrict__ pre, const float* __restrict__ net, int ld_net, float* __restrict__ z, float* __restrict__ rnet,
+// T = __half (half-operand gate convs): zr / q are the fp16 conv outputs and r*h goes into an fp16 RX; the state `net`,
+// z, bias and pre stay fp32, and gru_update writes the fp16 image of the new state into HX (h_img).
+template <typename T>
+__global__ void __launch_bounds__(256) k_gru_gate(const T* __restrict__ zr, const float* __restrict__ bias,
+    const float* __restrict__ pre, const float* __restrict__ net, int ld_net, float* __restrict__ z, T* __restrict__ rnet,
     int ld_r, long npix, int C) {
   const int c4n = C >> 2;
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= npix * c4n) return;
   const long pix = i / c4n; const int c = (int)(i - pix * c4n) * 4;
-  float4 zv = *reinterpret_cast<const float4*>(zr + pix * 2 * C + c), rv = *reinterpret_cast<const float4*>(zr + pix * 2 * C + C + c);
+  float4 zv = pp_ld4(zr + pix * 2 * C + c), rv = pp_ld4(zr + pix * 2 * C + C + c);
   float4 bz = make_float4(0.f, 0.f, 0.f, 0.f), br = bz;
   if (bias != nullptr) { bz = *reinterpret_cast<const float4*>(bias + c); br = *reinterpret_cast<const float4*>(bias + C + c); }
   if (pre != nullptr) {           // iteration-invariant part of the gate convs (context features), precomputed per pixel
@@ -613,16 +651,17 @@ __global__ void __launch_bounds__(256) k_gru_gate(const float* __restrict__ zr, 
   ro.x = h.x / (1.0f + expf(-(rv.x + br.x))); ro.y = h.y / (1.0f + expf(-(rv.y + br.y)));
   ro.z = h.z / (1.0f + expf(-(rv.z + br.z))); ro.w = h.w / (1.0f + expf(-(rv.w + br.w)));
   *reinterpret_cast<float4*>(z + pix * C + c) = zo;
-  *reinterpret_cast<float4*>(rnet + pix * ld_r + c) = ro;
+  pp_st4(rnet + pix * ld_r + c, ro);
 }
-__global__ void __launch_bounds__(256) k_gru_update(const float* __restrict__ q, const float* __restrict__ bias,
-    const float* __restrict__ pre, const float* __restrict__ z, float* __restrict__ net, int ld_net, float* __restrict__ net_copy,
-    long npix, int C) {
+template <typename T>
+__global__ void __launch_bounds__(256) k_gru_update(const T* __restrict__ q, const float* __restrict__ bias,
+    const float* __restrict__ pre, const float* __restrict__ z, float* __restrict__ net, int ld_net, T* __restrict__ h_img,
+    int ld_img, T* __restrict__ net_copy, long npix, int C) {
   const int c4n = C >> 2;
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= npix * c4n) return;
   const long pix = i / c4n; const int c = (int)(i - pix * c4n) * 4;
-  float4 qv = *reinterpret_cast<const float4*>(q + pix * C + c), b = make_float4(0.f, 0.f, 0.f, 0.f);
+  float4 qv = pp_ld4(q + pix * C + c), b = make_float4(0.f, 0.f, 0.f, 0.f);
   if (bias != nullptr) b = *reinterpret_cast<const float4*>(bias + c);
   if (pre != nullptr) {
     const float4 pq = *reinterpret_cast<const float4*>(pre + pix * C + c);
@@ -633,13 +672,25 @@ __global__ void __launch_bounds__(256) k_gru_update(const float* __restrict__ q,
   h.x = (1.0f - zv.x) * h.x + zv.x * tanhf(qv.x + b.x); h.y = (1.0f - zv.y) * h.y + zv.y * tanhf(qv.y + b.y);
   h.z = (1.0f - zv.z) * h.z + zv.z * tanhf(qv.z + b.z); h.w = (1.0f - zv.w) * h.w + zv.w * tanhf(qv.w + b.w);
   *reinterpret_cast<float4*>(net + pix * ld_net + c) = h;
-  if (net_copy != nullptr) *reinterpret_cast<float4*>(net_copy + pix * C + c) = h;   // dense copy for the flow / mask heads
+  if (h_img != nullptr) pp_st4(h_img + pix * ld_img + c, h);
+  if (net_copy != nullptr) pp_st4(net_copy + pix * C + c, h);                    // dense copy for the flow / mask heads
 }
 // z = sigmoid(conv_z), r*h (update.py:47-49 / :54-56): zr = raw output of the fused z|r conv [npix][2C]
 extern "C" int pp_gru_gate(const float* zr, const float* bias, const float* pre, const float* net, int ld_net, float* z,
                            float* rnet, int ld_r, long npix, int C, cudaStream_t stream) {
   if (C % 4 || ld_net % 4 || ld_r % 4 || ((uintptr_t)pre & 15) || ((uintptr_t)bias & 15)) return PP_ERR_ALIGN;
-  k_gru_gate<<<pp_blocks(npix * (C / 4), 256), 256, 0, stream>>>(zr, bias, pre, net, ld_net, z, rnet, ld_r, npix, C);
+  k_gru_gate<float><<<pp_blocks(npix * (C / 4), 256), 256, 0, stream>>>(zr, bias, pre, net, ld_net, z, rnet, ld_r, npix, C);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+// the same with the fp16 gate conv output `zr` and an fp16 rnet slice (8-byte aligned rows); net, z, bias, pre fp32
+extern "C" int pp_gru_gate_f16(const void* zr, const float* bias, const float* pre, const float* net, int ld_net, float* z,
+                               void* rnet, int ld_r, long npix, int C, cudaStream_t stream) {
+  if (C % 4 || ld_net % 4 || ld_r % 4 || ((uintptr_t)zr & 7) || ((uintptr_t)rnet & 7) || ((uintptr_t)net & 15) ||
+      ((uintptr_t)z & 15) || ((uintptr_t)pre & 15) || ((uintptr_t)bias & 15))
+    return PP_ERR_ALIGN;
+  k_gru_gate<__half><<<pp_blocks(npix * (C / 4), 256), 256, 0, stream>>>((const __half*)zr, bias, pre, net, ld_net, z, (__half*)rnet,
+                                                                        ld_r, npix, C);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }
@@ -647,29 +698,52 @@ extern "C" int pp_gru_gate(const float* zr, const float* bias, const float* pre,
 extern "C" int pp_gru_update(const float* q, const float* bias, const float* pre, const float* z, float* net, int ld_net,
                              float* net_copy, long npix, int C, cudaStream_t stream) {
   if (C % 4 || ld_net % 4 || ((uintptr_t)net_copy & 15) || ((uintptr_t)pre & 15) || ((uintptr_t)bias & 15)) return PP_ERR_ALIGN;
-  k_gru_update<<<pp_blocks(npix * (C / 4), 256), 256, 0, stream>>>(q, bias, pre, z, net, ld_net, net_copy, npix, C);
+  k_gru_update<float><<<pp_blocks(npix * (C / 4), 256), 256, 0, stream>>>(q, bias, pre, z, net, ld_net, nullptr, 0, net_copy, npix, C);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+// the same with the fp16 candidate conv output `q`: the fp32 state `net` is updated in place and its fp16 image is written
+// to h_img (ld_img; the state slice of HX, nullable) and net_copy (dense, nullable)
+extern "C" int pp_gru_update_f16(const void* q, const float* bias, const float* pre, const float* z, float* net, int ld_net,
+                                 void* h_img, int ld_img, void* net_copy, long npix, int C, cudaStream_t stream) {
+  if (C % 4 || ld_net % 4 || ld_img % 4 || ((uintptr_t)q & 7) || ((uintptr_t)h_img & 7) || ((uintptr_t)net_copy & 7) ||
+      ((uintptr_t)net & 15) || ((uintptr_t)z & 15) || ((uintptr_t)pre & 15) || ((uintptr_t)bias & 15))
+    return PP_ERR_ALIGN;
+  k_gru_update<__half><<<pp_blocks(npix * (C / 4), 256), 256, 0, stream>>>((const __half*)q, bias, pre, z, net, ld_net, (__half*)h_img,
+                                                                          ld_img, (__half*)net_copy, npix, C);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }
 // motion features [out(126) | flow(2)] (update.py:95-97) written into the same channel slot of two buffers
-__global__ void __launch_bounds__(256) k_raft_pack_motion(const float* __restrict__ mot, int ld_mot, const float* __restrict__ bias,
-    const float* __restrict__ flow, float* __restrict__ d0, float* __restrict__ d1, int ld, long npix) {
+template <typename T>
+__global__ void __launch_bounds__(256) k_raft_pack_motion(const T* __restrict__ mot, int ld_mot, const float* __restrict__ bias,
+    const float* __restrict__ flow, T* __restrict__ d0, T* __restrict__ d1, int ld, long npix) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;   // 32 float4 per pixel (128 channels)
   if (i >= npix * 32) return;
   const long pix = i >> 5; const int c = (int)(i & 31) * 4;
-  float4 v = *reinterpret_cast<const float4*>(mot + pix * ld_mot + c);
+  float4 v = pp_ld4(mot + pix * ld_mot + c);
   if (bias != nullptr) {                                        // raw conv output: bias + ReLU of update.py:96 applied here
     const float4 b = *reinterpret_cast<const float4*>(bias + c);
     v.x = fmaxf(v.x + b.x, 0.f); v.y = fmaxf(v.y + b.y, 0.f); v.z = fmaxf(v.z + b.z, 0.f); v.w = fmaxf(v.w + b.w, 0.f);
   }
   if (c == 124) { v.z = flow[2 * pix]; v.w = flow[2 * pix + 1]; }
-  *reinterpret_cast<float4*>(d0 + pix * ld + c) = v;
-  *reinterpret_cast<float4*>(d1 + pix * ld + c) = v;
+  pp_st4(d0 + pix * ld + c, v);
+  pp_st4(d1 + pix * ld + c, v);
 }
 extern "C" int pp_raft_pack_motion(const float* mot, int ld_mot, const float* bias, const float* flow, float* d0, float* d1,
                                    int ld, long npix, cudaStream_t stream) {
   if (ld % 4 || ld_mot % 4 || ((uintptr_t)bias & 15)) return PP_ERR_ALIGN;
-  k_raft_pack_motion<<<pp_blocks(npix * 32, 256), 256, 0, stream>>>(mot, ld_mot, bias, flow, d0, d1, ld, npix);
+  k_raft_pack_motion<float><<<pp_blocks(npix * 32, 256), 256, 0, stream>>>(mot, ld_mot, bias, flow, d0, d1, ld, npix);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+// the same from the fp16 motion conv output into fp16 HX / RX slots (8-byte aligned rows); bias and flow fp32
+extern "C" int pp_raft_pack_motion_f16(const void* mot, int ld_mot, const float* bias, const float* flow, void* d0, void* d1, int ld,
+                                       long npix, cudaStream_t stream) {
+  if (ld % 4 || ld_mot % 4 || ((uintptr_t)mot & 7) || ((uintptr_t)d0 & 7) || ((uintptr_t)d1 & 7) || ((uintptr_t)bias & 15))
+    return PP_ERR_ALIGN;
+  k_raft_pack_motion<__half><<<pp_blocks(npix * 32, 256), 256, 0, stream>>>((const __half*)mot, ld_mot, bias, flow, (__half*)d0,
+                                                                            (__half*)d1, ld, npix);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }

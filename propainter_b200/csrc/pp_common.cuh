@@ -81,4 +81,24 @@ static inline int pp_num_sms() {
   return n;
 }
 #define PP_NUM_SMS pp_num_sms()
+
+// fp32 or fp16 pixel-major rows for the elementwise kernels around the half-operand library convs (DESIGN.md §4
+// "Precision"): 4 consecutive channels in as float4 (fp16 rows: 8-byte aligned), out rounded to nearest.
+#include <cuda_fp16.h>
+__device__ __forceinline__ float4 pp_ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+__device__ __forceinline__ float4 pp_ld4(const __half* p) {
+  const uint2 u = *reinterpret_cast<const uint2*>(p);
+  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ void pp_st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
+__device__ __forceinline__ void pp_st4(__half* p, float4 v) {
+  const __half2 a = __floats2half2_rn(v.x, v.y), b = __floats2half2_rn(v.z, v.w);
+  uint2 u;
+  u.x = *reinterpret_cast<const uint32_t*>(&a);
+  u.y = *reinterpret_cast<const uint32_t*>(&b);
+  *reinterpret_cast<uint2*>(p) = u;
+}
+__device__ __forceinline__ void pp_st1(float* p, float v) { *p = v; }
+__device__ __forceinline__ void pp_st1(__half* p, float v) { *p = __float2half_rn(v); }
 #endif

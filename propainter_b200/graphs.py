@@ -14,7 +14,7 @@ from . import config, ops
 def _switches():
     """execution switches that are baked into a capture: part of the cache key, so flipping one re-captures"""
     return (config.LINEAR_TF32, config.FUSED_EPILOGUE, config.AUTOTUNE, config.CUDNN_BENCHMARK, config.UMMA_CONV, config.SCAN_PRIORITY,
-            torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
+            config.HALF_OPERANDS, torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
 
 
 _hp_streams = {}

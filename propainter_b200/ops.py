@@ -1,5 +1,6 @@
 """Tensor-level wrappers over the C ABI.  Each takes/returns torch CUDA tensors, passes raw pointers +
-the current stream, and raises on any non-zero return code.  fp32 only (DESIGN.md §6)."""
+the current stream, and raises on any non-zero return code.  fp32, except the fp16 operand / result tensors of RAFT's
+half-precision refinement convs (corr_lookup, bias_act, gru_gate, gru_update, raft_pack_motion; DESIGN.md §4 "Precision")."""
 import collections
 import ctypes
 import math
@@ -40,7 +41,7 @@ def _dense(t):
     return t
 
 
-def _pm(t):
+def _pm(t, dtype=torch.float32):
     """pixel-major view [..., C] whose pixels are `ld` elements apart -> (ptr, ld)."""
     if t.stride(-1) != 1:
         raise RuntimeError("channel dim must be unit-stride")
@@ -50,7 +51,7 @@ def _pm(t):
         if t.shape[d] != 1 and t.stride(d) != exp:
             raise RuntimeError("pixel-major view must be dense over its pixels")
         exp *= t.shape[d]
-    return _p(t), ld
+    return _p(t, dtype), ld
 
 
 def corr_ld(w):
@@ -82,10 +83,17 @@ def corr_build(fmap, idx1, idx2, levels, h, w):
 
 
 def corr_lookup(levels, coords, out=None, tma=True):
-    """coords [B,h,w,2] -> [B,h,w,324].  tma=False selects the plain-load baseline kernel."""
+    """coords [B,h,w,2] -> [B,h,w,324].  tma=False selects the plain-load baseline kernel.  An fp16 `out` [B,h,w,ld >= 324]
+    receives the taps rounded to nearest in channels [0, 324) of its rows."""
     B, h, w, _ = coords.shape
     if out is None:
         out = torch.empty(B, h, w, 324, device=coords.device, dtype=torch.float32)
+    if out.dtype == torch.float16:
+        fn = _lib.lib().pp_corr_lookup_f16 if tma else _lib.lib().pp_corr_lookup_ldg_f16
+        check(fn(_level_array(levels), _p(_dense(coords)), _p(_dense(out), torch.float16), out.shape[-1], B, h, w, _stream()),
+              "pp_corr_lookup_f16")
+        _count(1)
+        return out
     fn = _lib.lib().pp_corr_lookup if tma else _lib.lib().pp_corr_lookup_ldg
     check(fn(_level_array(levels), _p(_dense(coords)), _p(_dense(out)), B, h, w, _stream()), "pp_corr_lookup")
     _count(1)
@@ -419,19 +427,36 @@ def ffn_overlap_add(Y, frames, h, w, CH=40):
 
 def gru_gate(zr_pm, bias, net_view, z_out, rnet_view, pre=None):
     """zr_pm [..,2C] raw gate conv output; net_view / rnet_view: C-channel slices of HX / RX; z_out dense [..,C];
-    bias [2C] / pre [..,2C] optional addends."""
+    bias [2C] / pre [..,2C] optional addends.  fp16 zr_pm: rnet_view is fp16 too, net_view the fp32 state."""
     C = z_out.shape[-1]
     np_, ldn = _pm(net_view)
+    if zr_pm.dtype == torch.float16:
+        rp, ldr = _pm(rnet_view, torch.float16)
+        check(_lib.lib().pp_gru_gate_f16(_p(_dense(zr_pm), torch.float16), _p(bias), _p(_dense(pre)) if pre is not None else None, np_,
+                                         ldn, _p(_dense(z_out)), rp, ldr, z_out.numel() // C, C, _stream()), "pp_gru_gate_f16")
+        _count(1)
+        return
     rp, ldr = _pm(rnet_view)
     check(_lib.lib().pp_gru_gate(_p(_dense(zr_pm)), _p(bias), _p(_dense(pre)) if pre is not None else None, np_, ldn,
                                  _p(_dense(z_out)), rp, ldr, z_out.numel() // C, C, _stream()), "pp_gru_gate")
     _count(1)
 
 
-def gru_update(q_pm, bias, z, net_view, net_copy=None, pre=None):
-    """h = (1-z)*h + z*tanh(q+bias+pre) in place on the state slice; `net_copy` (dense) also receives h."""
+def gru_update(q_pm, bias, z, net_view, net_copy=None, pre=None, h_img=None):
+    """h = (1-z)*h + z*tanh(q+bias+pre) in place on the state slice; `net_copy` (dense) also receives h.  fp16 q_pm: the
+    state net_view stays fp32, its fp16 image goes to h_img (a C-channel slice of the fp16 HX) and the fp16 net_copy."""
     C = z.shape[-1]
     np_, ldn = _pm(net_view)
+    if q_pm.dtype == torch.float16:
+        ip, ldi = _pm(h_img, torch.float16) if h_img is not None else (None, C)
+        check(_lib.lib().pp_gru_update_f16(_p(_dense(q_pm), torch.float16), _p(bias), _p(_dense(pre)) if pre is not None else None,
+                                           _p(_dense(z)), np_, ldn, ip, ldi,
+                                           _p(_dense(net_copy), torch.float16) if net_copy is not None else None, z.numel() // C, C,
+                                           _stream()), "pp_gru_update_f16")
+        _count(1)
+        return
+    if h_img is not None:
+        raise RuntimeError("gru_update: h_img is the fp16 image of the state (fp16 q_pm only)")
     check(_lib.lib().pp_gru_update(_p(_dense(q_pm)), _p(bias), _p(_dense(pre)) if pre is not None else None, _p(_dense(z)), np_, ldn,
                                    _p(_dense(net_copy)) if net_copy is not None else None, z.numel() // C, C, _stream()),
           "pp_gru_update")
@@ -440,12 +465,18 @@ def gru_update(q_pm, bias, z, net_view, net_copy=None, pre=None):
 
 def raft_pack_motion(mot_pm, flow_pm, d0_view, d1_view, bias=None):
     """mot_pm [..,128] (channels 126,127 ignored), flow_pm [..,2] -> 128-channel slot views of HX and RX.
-    With `bias`, mot_pm is the raw conv output and relu(mot + bias) is applied on the way."""
-    mp, ldm = _pm(mot_pm)
-    p0, ld0 = _pm(d0_view)
-    p1, ld1 = _pm(d1_view)
+    With `bias`, mot_pm is the raw conv output and relu(mot + bias) is applied on the way.  fp16 mot_pm: fp16 HX / RX."""
+    dt = mot_pm.dtype
+    mp, ldm = _pm(mot_pm, dt)
+    p0, ld0 = _pm(d0_view, dt)
+    p1, ld1 = _pm(d1_view, dt)
     if ld0 != ld1:
         raise RuntimeError("HX / RX must share the pixel stride")
+    if dt == torch.float16:
+        check(_lib.lib().pp_raft_pack_motion_f16(mp, ldm, _p(bias), _p(_dense(flow_pm)), p0, p1, ld0, flow_pm.numel() // 2, _stream()),
+              "pp_raft_pack_motion_f16")
+        _count(1)
+        return
     check(_lib.lib().pp_raft_pack_motion(mp, ldm, _p(bias), _p(_dense(flow_pm)), p0, p1, ld0, flow_pm.numel() // 2, _stream()),
           "pp_raft_pack_motion")
     _count(1)
@@ -471,11 +502,24 @@ ACT = {"none": 0, "relu": 1, "leaky": 2, "sigmoid": 3, "tanh": 4}
 
 def bias_act(x_pm, bias=None, act="none", slope=0.0, res=None, post_relu=False, out=None, pre=None):
     """out = post(act(x + bias + pre) + res) on pixel-major views [..., C] (unit channel stride, dense over pixels; x / pre /
-    res / out may each be a channel slice of a wider buffer).  out=None -> in place on x_pm.  Returns out."""
+    res / out may each be a channel slice of a wider buffer).  out=None -> in place on x_pm.  Returns out.  x_pm and out may
+    be fp16 (RAFT's half-precision refinement convs); bias / pre / res and the arithmetic are fp32."""
     C = x_pm.shape[-1]
     out = x_pm if out is None else out
     if out.shape != x_pm.shape or (res is not None and res.shape != x_pm.shape) or (pre is not None and pre.shape != x_pm.shape):
         raise RuntimeError("bias_act: shape mismatch")
+    if torch.float16 in (x_pm.dtype, out.dtype):
+        if not {x_pm.dtype, out.dtype} <= {torch.float16, torch.float32}:
+            raise RuntimeError(f"bias_act: x / out must be fp32 or fp16, got {x_pm.dtype} / {out.dtype}")
+        xp, ldx = _pm(x_pm, x_pm.dtype)
+        op, ldo = _pm(out, out.dtype)
+        rp, ldr = _pm(res) if res is not None else (None, C)
+        pp, ldp = _pm(pre) if pre is not None else (None, C)
+        check(_lib.lib().pp_bias_act_f16(xp, ldx, int(x_pm.dtype == torch.float16), _p(bias), pp, ldp, rp, ldr, op, ldo,
+                                         int(out.dtype == torch.float16), x_pm.numel() // C, C, ACT[act], float(slope),
+                                         int(bool(post_relu)), _stream()), "pp_bias_act_f16")
+        _count(1)
+        return out
     xp, ldx = _pm(x_pm)
     op, ldo = _pm(out)
     rp, ldr = _pm(res) if res is not None else (None, C)
