@@ -294,6 +294,23 @@ int pp_flow_maxrad(const float* flow, float* maxima, int N, int H, int W, int pe
  * pp_flow_maxrad with the matching per_frame -> uint8 out [N][H][W][3], RGB (BGR when bgr). */
 int pp_flow_to_image_u8(const float* flow, const float* maxima, uint8_t* out, int N, int H, int W, int variant, int has_clip,
                         float clip_flow, int bgr, cudaStream_t stream);
+/* ---- I3D feature network of VFID (core/metrics.py:62-82,195-569) ---------------------------------------------- */
+/* 'same' padding (Unit3D / MaxPool3dSamePadding.compute_pad, core/metrics.py:196-200,258-262): for a k-tap window of stride
+ * s over n samples, pad = max(k - (n % s ? n % s : s), 0), front pad / 2, back the rest (pp_same_pad in pp_elem.cuh);
+ * the output extent is (n + pad - k) / s + 1. */
+/* to_tensors (core/utils.py:151-170) + transpose(1, 2) (core/metrics.py:183) + the F.pad of Conv3d_1a_7x7
+ * (core/metrics.py:264-279, k = 7, s = 2 per axis): src uint8 frames [B][T][H][W][3] (src_u8 != 0, value u8 / 255) or
+ * planar float [B][3][T][H][W] (src_u8 == 0, copied) -> dst float [B][T+pt][H+ph][W+pw][4] (16-byte aligned), zero
+ * border and a zero 4th channel; conv1a then runs with padding 0. */
+int pp_i3d_input(const void* src, int src_u8, float* dst, int B, int T, int H, int W, cudaStream_t stream);
+/* MaxPool3dSamePadding (core/metrics.py:195-218): F.pad with zeros + nn.MaxPool3d((kt,kh,kw), (st,sh,sw)), NaN
+ * propagating as ATen's max pooling does.  x [B][T][H][W][ld_x] -> out [B][To][Ho][Wo][ld_out] (channels [0, C) of its
+ * rows, so out may be a channel slice); C, ld_x, ld_out multiples of 4, 16-byte aligned pointers. */
+int pp_maxpool3d_same(const float* x, int ld_x, float* out, int ld_out, int B, int T, int H, int W, int C, int kt, int kh, int kw,
+                      int st, int sh, int sw, cudaStream_t stream);
+/* x.mean(4).mean(3).mean(2) of extract_features(target_endpoint='Logits') (core/metrics.py:566-567): x [B][N][ld]
+ * (N = T*H*W pixels) -> out float [B][C], summed in float64 in a fixed order and rounded once. */
+int pp_mean_thw(const float* x, int ld, float* out, int B, long N, int C, cudaStream_t stream);
 
 #ifdef __cplusplus
 }

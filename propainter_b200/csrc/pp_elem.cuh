@@ -459,3 +459,17 @@ PP_HD void pp_flowviz_pt(float u, float v, float den, int bgr, uint8_t* rgb) {
     rgb[bgr ? 2 - c : c] = (uint8_t)(int)floorf(PP_MUL(255.0f, col));
   }
 }
+
+// ---- I3D (core/metrics.py:195-569) ----
+// TF 'same' padding of a k-tap, stride-s window over n samples: Unit3D.compute_pad / MaxPool3dSamePadding.compute_pad
+// (core/metrics.py:196-200,258-262).  The front takes pad / 2, the back the rest, so even pads of 5 split 2 / 3.
+PP_HD int pp_same_pad(int k, int s, int n) {
+  const int r = n % s;
+  const int p = r == 0 ? k - s : k - r;
+  return p > 0 ? p : 0;
+}
+// output extent of that window: ceil(n / s) for every (k, s) I3D uses
+PP_HD int pp_same_out(int k, int s, int n) { return (n + pp_same_pad(k, s, n) - k) / s + 1; }
+// one tap of ATen's max pooling (max_pool3d_with_indices): a larger value or a NaN replaces the running maximum, so
+// the first NaN sticks and, among equal values (+0 / -0), the first tap in (t, y, x) order wins
+PP_HD float pp_pool_max(float m, float v) { return (v > m || isnan(v)) ? v : m; }

@@ -8,9 +8,15 @@ PSNR: 20 log10(255 / sqrt(MSE)) over float64 (core/metrics.py:20-36).  SSIM: ski
 multichannel=True, win_size=65) as core/metrics.py:44-47 calls it -- uniform 65x65 windows, sample covariance
 (N/(N-1)), K1 = 0.01, K2 = 0.03, mean over the positions whose window lies inside the image and over the channels; restated
 from scikit-image's published `structural_similarity` (third-party dependency, not installed here; pinned against a direct
-numpy evaluation of the same definition in tests/test_evaluate.py).  VFID needs the I3D checkpoint
-(core/metrics.py:55-120), which does not exist in the build environment: `i3d_activations` is accepted as a callable so
-the reference's I3D can be plugged in, and FID is then computed as core/metrics.py:122-160 does."""
+numpy evaluation of the same definition in tests/test_evaluate.py).  VFID: `evaluate_clip` takes an `i3d_activations`
+callable; `i3d_activations(model, frames_u8)` below is the reference's calculate_i3d_activations (core/metrics.py:70-82)
+on this package's InceptionI3d (propainter_b200.model.i3d), and `video_completion_summary` gives the script's final
+PSNR / SSIM / VFID line, FID computed as core/metrics.py:85-150 does.
+
+    i3d = InceptionI3d(400, in_channels=3, final_endpoint='Logits').to("cuda")
+    i3d.load_state_dict(torch.load("weights/i3d_rgb_imagenet.pt"), strict=True)
+    res = [evaluate_clip(pipe, f, m, i3d_activations=functools.partial(i3d_activations, i3d)) for f, m in clips]
+    video_completion_summary(res)                         # {"psnr", "ssim", "vfid", "seconds_per_frame", "videos"}"""
 import time
 
 import numpy as np
@@ -84,6 +90,38 @@ def evaluate_clip(pipe, frames_u8, masks_u8, cfg=None, mask_dilation=0, i3d_acti
            "psnr_per_frame": ps.tolist(), "ssim_per_frame": ss.tolist(), "seconds": dt, "frames_per_s": fr.shape[0] / dt, "comp": comp}
     if i3d_activations is not None:
         out["i3d"] = (i3d_activations(fr), i3d_activations(comp))
+    return out
+
+
+@torch.no_grad()
+def i3d_activations(model, frames_u8):
+    """calculate_i3d_activations (core/metrics.py:70-82) for one video: uint8 frames [T,H,W,3] (numpy or tensor) -> float32
+    numpy [1024], the I3D features of the to_tensors video on `model`'s device.  A batch [B,T,H,W,3] of equally long
+    videos -> [B,1024] in one pass (eval BatchNorm is per sample, so a row does not depend on the others beyond the
+    rounding of the convolution algorithm cuDNN picks for that batch size)."""
+    fr = torch.as_tensor(frames_u8)
+    single = fr.dim() == 4
+    fr = fr[None] if single else fr
+    if fr.dtype != torch.uint8:
+        raise ValueError(f"i3d_activations: expected uint8 frames, got {fr.dtype}")
+    feats = model.features_u8(fr.to(model.device).contiguous()).cpu().numpy()
+    return feats[0] if single else feats
+
+
+def video_completion_summary(results):
+    """The final line of scripts/evaluate_propainter.py:245-251 over evaluate_clip results (each with its "i3d" pair):
+    PSNR and SSIM averaged over all frames of all videos (total_frame_psnr / total_frame_ssim, so an identical frame's inf
+    carries through), VFID = calculate_vfid of the stacked per-video activations (core/metrics.py:85-96), and the mean over
+    videos of seconds per frame (time_all)."""
+    psnr = [p for r in results for p in r["psnr_per_frame"]]
+    ssim = [s for r in results for s in r["ssim_per_frame"]]
+    out = {"psnr": sum(psnr) / len(psnr), "ssim": sum(ssim) / len(ssim),
+           "seconds_per_frame": sum(r["seconds"] / len(r["psnr_per_frame"]) for r in results) / len(results),
+           "videos": len(results)}
+    if all("i3d" in r for r in results):
+        real = np.stack([np.asarray(r["i3d"][0]) for r in results])
+        fake = np.stack([np.asarray(r["i3d"][1]) for r in results])
+        out["vfid"] = fid_from_activations(real, fake)
     return out
 
 

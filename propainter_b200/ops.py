@@ -682,6 +682,70 @@ def flow_to_image_u8(flow, normalize="frame", clip_flow=None, bgr=False):
     return out[0] if single else out
 
 
+# ---------------------------------------------------------------- I3D feature network (VFID)
+def same_pad(k, s, n):
+    """TF 'same' padding of a k-tap, stride-s window over n samples (pp_same_pad, core/metrics.py:196-200,258-262); the front
+    gets pad // 2."""
+    p = k - (n % s if n % s else s)
+    return max(p, 0)
+
+
+def same_out(k, s, n):
+    """output extent of that window (pp_same_out)"""
+    return (n + same_pad(k, s, n) - k) // s + 1
+
+
+def i3d_input(video):
+    """Conv3d_1a_7x7's padded operand: uint8 frames [B,T,H,W,3] (value u8 / 255, as to_tensors) or planar float32
+    [B,3,T,H,W] (copied) -> float32 [B,T+pt,H+ph,W+pw,4] with the asymmetric 'same' border of a 7-tap stride-2 window
+    and a zero 4th channel."""
+    if video.dim() != 5:
+        raise RuntimeError(f"i3d_input: expected a 5-d video, got {tuple(video.shape)}")
+    u8 = video.dtype == torch.uint8
+    if u8:
+        if video.shape[-1] != 3:
+            raise RuntimeError("i3d_input: uint8 frames must be [B,T,H,W,3]")
+        B, T, H, W, _ = video.shape
+    else:
+        if video.shape[1] != 3:
+            raise RuntimeError("i3d_input: float video must be [B,3,T,H,W]")
+        B, _, T, H, W = video.shape
+    src = _p(_dense(video), video.dtype if u8 else torch.float32)
+    out = torch.empty(B, T + same_pad(7, 2, T), H + same_pad(7, 2, H), W + same_pad(7, 2, W), 4, device=video.device,
+                      dtype=torch.float32)
+    check(_lib.lib().pp_i3d_input(src, int(u8), _p(out), B, T, H, W, _stream()), "pp_i3d_input")
+    _count(1)
+    return out
+
+
+def maxpool3d_same(x, kernel, stride, out=None):
+    """MaxPool3dSamePadding (core/metrics.py:195-218) on a pixel-major map x [B,T,H,W,C] (dense pixels, C a multiple of 4)
+    -> out [B,To,Ho,Wo,C] (may be a channel slice of a wider buffer).  Padded taps count as zeros, as after F.pad."""
+    B, T, H, W, C = x.shape
+    (kt, kh, kw), (st, sh, sw) = kernel, stride
+    shape = (B, same_out(kt, st, T), same_out(kh, sh, H), same_out(kw, sw, W), C)
+    if out is None:
+        out = torch.empty(shape, device=x.device, dtype=torch.float32)
+    if tuple(out.shape) != shape:
+        raise RuntimeError(f"maxpool3d_same: out {tuple(out.shape)} != {shape}")
+    xp, ldx = _pm(x)
+    op, ldo = _pm(out)
+    check(_lib.lib().pp_maxpool3d_same(xp, ldx, op, ldo, B, T, H, W, C, kt, kh, kw, st, sh, sw, _stream()), "pp_maxpool3d_same")
+    _count(1)
+    return out
+
+
+def mean_thw(x):
+    """x.mean(4).mean(3).mean(2) of an NCDHW map, on its pixel-major form x [B,T,H,W,C] -> float32 [B,C]: float64
+    fixed-order sums, rounded once."""
+    B, C = x.shape[0], x.shape[-1]
+    xp, ld = _pm(x)
+    out = torch.empty(B, C, device=x.device, dtype=torch.float32)
+    check(_lib.lib().pp_mean_thw(xp, ld, _p(out), B, x[0, ..., 0].numel(), C, _stream()), "pp_mean_thw")
+    _count(1)
+    return out
+
+
 # ---------------------------------------------------------------- resizing around the path (tables on the host, passes on the device)
 _TABLES = {}
 

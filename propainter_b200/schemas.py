@@ -7,6 +7,7 @@ GEN :  model/propainter.py:34-54,72-101,193-216,235-304; model/modules/sparse_tr
 The golden manifest ``tests/golden/state_dict_manifest.json`` (dumped from the reference modules in
 the authoring container) pins these in the CPU test-suite; ``tests/golden/state_dict_manifest_raft_small.json`` pins
 ``raft_small_schema``.
+I3D (the VFID feature network): core/metrics.py:221-256,289-531, pinned by ``tests/golden/state_dict_manifest_i3d.json``.
 """
 import torch
 
@@ -80,6 +81,51 @@ def raft_small_schema():
         S.conv(f"{u}gru.conv{gate}", 96 + 146, 96, 3)
     S.conv(u + "flow_head.conv1", 96, 128, 3, gain=1.4)
     S.conv(u + "flow_head.conv2", 128, 2, 3, gain=0.05)   # keeps random-init flow within a few px
+    return S
+
+
+# InceptionI3d's Inception blocks (core/metrics.py:449-517): name, input channels, (b0, b1a, b1b, b2a, b2b, b3b) outputs.
+# The pooling endpoints between them carry no parameters.
+I3D_INCEPTION = (
+    ("Mixed_3b", 192, (64, 96, 128, 16, 32, 32)),
+    ("Mixed_3c", 256, (128, 128, 192, 32, 96, 64)),
+    ("Mixed_4b", 480, (192, 96, 208, 16, 48, 64)),
+    ("Mixed_4c", 512, (160, 112, 224, 24, 64, 64)),
+    ("Mixed_4d", 512, (128, 128, 256, 24, 64, 64)),
+    ("Mixed_4e", 512, (112, 144, 288, 32, 64, 64)),
+    ("Mixed_4f", 528, (256, 160, 320, 32, 128, 128)),
+    ("Mixed_5b", 832, (256, 160, 320, 32, 128, 128)),
+    ("Mixed_5c", 832, (384, 192, 384, 48, 128, 128)),
+)
+
+
+def _unit3d(S, p, cin, cout, k):
+    """Unit3D (core/metrics.py:221-256): bias-free conv3d + BatchNorm3d(eps=1e-3).  Seeded init: Kaiming-normal conv weights
+    (ReLU gain) so the signal survives 57 layers, and BN statistics / affine spread so that folding them is exercised."""
+    S.conv(p + ".conv3d", cin, cout, k, bias=False, nd=3, gain=2 ** 0.5)
+    S.add(p + ".bn.weight", (cout,), init=("uniform", 0.5, 1.5))
+    S.add(p + ".bn.bias", (cout,), init=("normal", 0.1))
+    S.add(p + ".bn.running_mean", (cout,), kind="buffer", init=("normal", 0.1))
+    S.add(p + ".bn.running_var", (cout,), kind="buffer", init=("uniform", 0.5, 2.0))
+    S.add(p + ".bn.num_batches_tracked", (), kind="buffer", dtype=torch.int64, init=("zeros",))
+
+
+def i3d_schema(num_classes=400, in_channels=3):
+    """InceptionI3d(final_endpoint='Logits') core/metrics.py:334-531 in its state_dict order: `logits` first (it is assigned
+    in __init__ before build() registers the endpoints), then the endpoints; the unused classifier head stays so that
+    pytorch-i3d checkpoints load strict."""
+    S = Schema()
+    S.conv("logits.conv3d", 1024, num_classes, 1, nd=3)
+    _unit3d(S, "Conv3d_1a_7x7", in_channels, 64, 7)
+    _unit3d(S, "Conv3d_2b_1x1", 64, 64, 1)
+    _unit3d(S, "Conv3d_2c_3x3", 64, 192, 3)
+    for name, cin, (c0, c1a, c1b, c2a, c2b, c3b) in I3D_INCEPTION:
+        _unit3d(S, name + ".b0", cin, c0, 1)
+        _unit3d(S, name + ".b1a", cin, c1a, 1)
+        _unit3d(S, name + ".b1b", c1a, c1b, 3)
+        _unit3d(S, name + ".b2a", cin, c2a, 1)
+        _unit3d(S, name + ".b2b", c2a, c2b, 3)
+        _unit3d(S, name + ".b3b", cin, c3b, 1)
     return S
 
 
