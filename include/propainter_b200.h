@@ -33,7 +33,7 @@ int pp_corr_build(const float* fmap, int D, const int* idx1, const int* idx2, in
  * 4 device pointers); level 0 must be filled. */
 int pp_corr_pool_pyramid(float* const* levels, long planes, int h, int w, cudaStream_t stream);
 /* CorrBlock.__call__ :29-50 + bilinear_sampler RAFT/utils/utils.py:57-71.
- * coords [n_pairs*h*w][2] (x,y) -> out pixel-major [n_pairs*h*w][324]. */
+ * coords [n_pairs*h*w][2] (x,y) -> out pixel-major [n_pairs*h*w][324].  n_pairs = 0 returns PP_OK without a launch. */
 int pp_corr_lookup(const float* const* levels, const float* coords, float* out, long n_pairs, int h, int w,
                    cudaStream_t stream);
 /* same contract, plain global loads instead of TMA staging (baseline for the ncu comparison) */
@@ -185,6 +185,8 @@ int pp_add_layernorm(const float* x, const float* delta, const float* gamma, con
                      int C, float eps, cudaStream_t stream);
 
 /* ---- RAFT SepConvGRU elementwise fusion (RAFT/update.py:45-60,95-97) ------------------------- */
+/* All of them read and write 4 channels at a time: every fp32 pointer must be 16-byte aligned and every stride a multiple
+ * of 4 (else PP_ERR_ALIGN, checked before anything is launched); npix = 0 returns PP_OK without a launch. */
 /* zr: raw output of the fused z|r gate conv [npix][2C]; net: state slice of HX (ld_net); writes z [npix][C]
  * and r*net into the state slice of RX (ld_r).  bias [2C] and pre [npix][2C] are nullable addends: `pre` carries the
  * part of the gate convs that does not change over the refinement iterations (the context-feature input channels,

@@ -126,6 +126,7 @@ template <int R, typename TO>
 static int corr_lookup_tma(const float* const* levels, const float* coords, TO* out, int ld_out, long n_pairs, int h, int w,
                            cudaStream_t stream) {
   if ((h >> 3) < 2 || (w >> 3) < 2) return PP_ERR_SHAPE;
+  if (n_pairs <= 0) return PP_OK;          // nothing to look up: no tensor maps, no zero-block launch
   const long npix = n_pairs * h * w;
   if (npix > 0x7fffffffL) return PP_ERR_SHAPE;
   PFN_encodeTiled enc = lk_encoder();

@@ -226,6 +226,7 @@ template <int R, typename TO>
 static int corr_lookup_ldg(const float* const* levels, const float* coords, TO* out, int ld_out, long n_pairs, int h, int w,
                            cudaStream_t stream) {
   if ((h >> 3) < 2 || (w >> 3) < 2) return PP_ERR_SHAPE;
+  if (n_pairs <= 0) return PP_OK;          // a zero-block grid would leave a launch error behind for the next kernel
   PPLevels lv;
   for (int l = 0; l < 4; ++l) lv.p[l] = levels[l];
   const long npix = n_pairs * h * w;
@@ -678,7 +679,10 @@ __global__ void __launch_bounds__(256) k_gru_update(const T* __restrict__ q, con
 // z = sigmoid(conv_z), r*h (update.py:47-49 / :54-56): zr = raw output of the fused z|r conv [npix][2C]
 extern "C" int pp_gru_gate(const float* zr, const float* bias, const float* pre, const float* net, int ld_net, float* z,
                            float* rnet, int ld_r, long npix, int C, cudaStream_t stream) {
-  if (C % 4 || ld_net % 4 || ld_r % 4 || ((uintptr_t)pre & 15) || ((uintptr_t)bias & 15)) return PP_ERR_ALIGN;
+  if (C % 4 || ld_net % 4 || ld_r % 4 || ((uintptr_t)zr & 15) || ((uintptr_t)net & 15) || ((uintptr_t)z & 15) ||
+      ((uintptr_t)rnet & 15) || ((uintptr_t)pre & 15) || ((uintptr_t)bias & 15))
+    return PP_ERR_ALIGN;
+  if (npix <= 0) return PP_OK;
   k_gru_gate<float><<<pp_blocks(npix * (C / 4), 256), 256, 0, stream>>>(zr, bias, pre, net, ld_net, z, rnet, ld_r, npix, C);
   PP_LAUNCH_CHECK();
   return PP_OK;
@@ -689,6 +693,7 @@ extern "C" int pp_gru_gate_f16(const void* zr, const float* bias, const float* p
   if (C % 4 || ld_net % 4 || ld_r % 4 || ((uintptr_t)zr & 7) || ((uintptr_t)rnet & 7) || ((uintptr_t)net & 15) ||
       ((uintptr_t)z & 15) || ((uintptr_t)pre & 15) || ((uintptr_t)bias & 15))
     return PP_ERR_ALIGN;
+  if (npix <= 0) return PP_OK;
   k_gru_gate<__half><<<pp_blocks(npix * (C / 4), 256), 256, 0, stream>>>((const __half*)zr, bias, pre, net, ld_net, z, (__half*)rnet,
                                                                         ld_r, npix, C);
   PP_LAUNCH_CHECK();
@@ -697,7 +702,10 @@ extern "C" int pp_gru_gate_f16(const void* zr, const float* bias, const float* p
 // h = (1-z)*h + z*tanh(conv_q) in place (update.py:50-51 / :57-58); net_copy (nullable) also receives h densely
 extern "C" int pp_gru_update(const float* q, const float* bias, const float* pre, const float* z, float* net, int ld_net,
                              float* net_copy, long npix, int C, cudaStream_t stream) {
-  if (C % 4 || ld_net % 4 || ((uintptr_t)net_copy & 15) || ((uintptr_t)pre & 15) || ((uintptr_t)bias & 15)) return PP_ERR_ALIGN;
+  if (C % 4 || ld_net % 4 || ((uintptr_t)q & 15) || ((uintptr_t)z & 15) || ((uintptr_t)net & 15) || ((uintptr_t)net_copy & 15) ||
+      ((uintptr_t)pre & 15) || ((uintptr_t)bias & 15))
+    return PP_ERR_ALIGN;
+  if (npix <= 0) return PP_OK;
   k_gru_update<float><<<pp_blocks(npix * (C / 4), 256), 256, 0, stream>>>(q, bias, pre, z, net, ld_net, nullptr, 0, net_copy, npix, C);
   PP_LAUNCH_CHECK();
   return PP_OK;
@@ -709,6 +717,7 @@ extern "C" int pp_gru_update_f16(const void* q, const float* bias, const float* 
   if (C % 4 || ld_net % 4 || ld_img % 4 || ((uintptr_t)q & 7) || ((uintptr_t)h_img & 7) || ((uintptr_t)net_copy & 7) ||
       ((uintptr_t)net & 15) || ((uintptr_t)z & 15) || ((uintptr_t)pre & 15) || ((uintptr_t)bias & 15))
     return PP_ERR_ALIGN;
+  if (npix <= 0) return PP_OK;
   k_gru_update<__half><<<pp_blocks(npix * (C / 4), 256), 256, 0, stream>>>((const __half*)q, bias, pre, z, net, ld_net, (__half*)h_img,
                                                                           ld_img, (__half*)net_copy, npix, C);
   PP_LAUNCH_CHECK();
@@ -732,7 +741,9 @@ __global__ void __launch_bounds__(256) k_raft_pack_motion(const T* __restrict__ 
 }
 extern "C" int pp_raft_pack_motion(const float* mot, int ld_mot, const float* bias, const float* flow, float* d0, float* d1,
                                    int ld, long npix, cudaStream_t stream) {
-  if (ld % 4 || ld_mot % 4 || ((uintptr_t)bias & 15)) return PP_ERR_ALIGN;
+  if (ld % 4 || ld_mot % 4 || ((uintptr_t)mot & 15) || ((uintptr_t)d0 & 15) || ((uintptr_t)d1 & 15) || ((uintptr_t)bias & 15))
+    return PP_ERR_ALIGN;
+  if (npix <= 0) return PP_OK;
   k_raft_pack_motion<float><<<pp_blocks(npix * 32, 256), 256, 0, stream>>>(mot, ld_mot, bias, flow, d0, d1, ld, npix);
   PP_LAUNCH_CHECK();
   return PP_OK;
@@ -742,6 +753,7 @@ extern "C" int pp_raft_pack_motion_f16(const void* mot, int ld_mot, const float*
                                        long npix, cudaStream_t stream) {
   if (ld % 4 || ld_mot % 4 || ((uintptr_t)mot & 7) || ((uintptr_t)d0 & 7) || ((uintptr_t)d1 & 7) || ((uintptr_t)bias & 15))
     return PP_ERR_ALIGN;
+  if (npix <= 0) return PP_OK;
   k_raft_pack_motion<__half><<<pp_blocks(npix * 32, 256), 256, 0, stream>>>((const __half*)mot, ld_mot, bias, flow, (__half*)d0,
                                                                             (__half*)d1, ld, npix);
   PP_LAUNCH_CHECK();
