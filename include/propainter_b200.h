@@ -166,12 +166,22 @@ typedef struct PPAttnParams {
 int pp_sparse_window_attn(const PPAttnParams* prm, int n_windows, cudaStream_t stream);
 /* same contract; masked windows on the warp-level mma.sync kernel (baseline of the wgmma kernel) */
 int pp_sparse_window_attn_mma(const PPAttnParams* prm, int n_windows, cudaStream_t stream);
+/* same window / key-table semantics (incl. nkf = 0 and flags) on fp16 operands: qkv [t][NT][3C] and pool [t][NP][2C] fp16,
+ * out [t][NT][C] fp16 rounded to nearest; scores, softmax statistics and O accumulate in fp32 (Q is scaled in fp32 and rounded
+ * once).  Masked windows: wgmma m64nNk16 f32.f16.f16; unmasked windows: mma.sync m16n8k16.  Rows 16-byte aligned and
+ * ld_* % 8 == 0 (else PP_ERR_ALIGN); WN <= 48; t = 0 or n_windows = 0 returns PP_OK without a launch. */
+int pp_sparse_window_attn_f16(const PPAttnParams* prm, int n_windows, cudaStream_t stream);
 
 /* FusionFeedForward.forward model/modules/sparse_transformer.py:81-100: fold -> /normalizer -> unfold -> GELU.
  * Y,Z [frames*fh*fw][ld], hidden columns tap-major (tap*CH + c). */
 size_t pp_ffn_overlap_add_workspace_bytes(int frames, int h, int w, int CH);
 int pp_ffn_overlap_add(const float* Y, int ldy, float* Z, int ldz, int frames, int h, int w, int CH, void* workspace,
                        size_t ws_bytes, cudaStream_t stream);
+/* the same on fp16 Y and Z (the half-operand fc1 output and fc2 operand): rows 16-byte aligned, ldy % 8 == ldz % 8 == 0
+ * (else PP_ERR_ALIGN); the fold sums in fp32 in the same order into the fp32 workspace, Z is rounded to nearest once.
+ * frames = 0 returns PP_OK without a launch. */
+int pp_ffn_overlap_add_f16(const void* Y, int ldy, void* Z, int ldz, int frames, int h, int w, int CH, void* workspace,
+                           size_t ws_bytes, cudaStream_t stream);
 
 /* ---- transformer glue ------------------------------------------------------------------------ */
 /* SparseWindowAttention.pool_layer (model/modules/sparse_transformer.py:131-133, used :203-206): depthwise Conv2d with
@@ -179,10 +189,19 @@ int pp_ffn_overlap_add(const float* Y, int ldy, float* Z, int ldz, int frames, i
  * out [n][H/kh][W/kw][C] dense. */
 int pp_pool_depthwise(const float* x, int ld_x, const float* w_taps, const float* bias, float* out, int n, int H, int W, int C,
                       int kh, int kw, cudaStream_t stream);
+/* the same on fp16 x and out (the half-operand LayerNorm output and the pooled K/V Linear's operand): weights, bias and the
+ * sums fp32, out rounded to nearest; rows 16-byte aligned, C % 8 == ld_x % 8 == 0 (else PP_ERR_ALIGN); n = 0 returns PP_OK. */
+int pp_pool_depthwise_f16(const void* x, int ld_x, const float* w_taps, const float* bias, void* out, int n, int H, int W, int C,
+                          int kh, int kw, cudaStream_t stream);
 /* TemporalSparseTransformer.forward model/modules/sparse_transformer.py:322-334: x_out = x + delta (residual),
  * y = LayerNorm(x_out) * gamma + beta, rows of C in {128,256,512,1024} floats.  delta NULL: plain LayerNorm. */
 int pp_add_layernorm(const float* x, const float* delta, const float* gamma, const float* beta, float* x_out, float* y, long rows,
                      int C, float eps, cudaStream_t stream);
+/* the same with an fp16 delta (delta_f16 != 0: the half-operand fc2 output) and / or an fp16 y (y_f16 != 0: the operand of the
+ * half-operand fc1), rounded to nearest; x / x_out and the statistics stay fp32.  Rows 16-byte aligned (else PP_ERR_ALIGN);
+ * rows = 0 returns PP_OK without a launch. */
+int pp_add_layernorm_f16(const float* x, const void* delta, int delta_f16, const float* gamma, const float* beta, float* x_out,
+                         void* y, int y_f16, long rows, int C, float eps, cudaStream_t stream);
 
 /* ---- RAFT SepConvGRU elementwise fusion (RAFT/update.py:45-60,95-97) ------------------------- */
 /* All of them read and write 4 channels at a time: every fp32 pointer must be 16-byte aligned and every stride a multiple

@@ -80,9 +80,12 @@ SIGNATURES = {
     "pp_window_mask": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "pp_sparse_window_attn": (c_int, [ctypes.POINTER(PPAttnParams), c_int, c_void_p]),
     "pp_sparse_window_attn_mma": (c_int, [ctypes.POINTER(PPAttnParams), c_int, c_void_p]),
+    "pp_sparse_window_attn_f16": (c_int, [ctypes.POINTER(PPAttnParams), c_int, c_void_p]),
     "pp_ffn_overlap_add_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "pp_ffn_overlap_add": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t,
                                    c_void_p]),
+    "pp_ffn_overlap_add_f16": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t,
+                                       c_void_p]),
     "pp_gru_gate": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_long, c_int, c_void_p]),
     "pp_gru_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_long, c_int, c_void_p]),
     "pp_raft_pack_motion": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_long, c_void_p]),
@@ -99,6 +102,10 @@ SIGNATURES = {
                                 c_int, c_float, c_int, c_void_p]),
     "pp_pool_depthwise": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "pp_add_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_long, c_int, c_float, c_void_p]),
+    "pp_pool_depthwise_f16": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
+                                      c_void_p]),
+    "pp_add_layernorm_f16": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_long, c_int,
+                                     c_float, c_void_p]),
     "pp_instance_norm_workspace_bytes": (c_size_t, [c_int, c_long, c_int]),
     "pp_instance_norm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_long, c_int, c_float, c_int, c_int, c_void_p, c_size_t,
                                  c_void_p]),

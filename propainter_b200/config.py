@@ -24,6 +24,13 @@ HALF_OPERANDS   RAFT's refinement-loop convs (convc1, convc2, convf2, the motion
                 10 mantissa bits, so this replaces TF32 by the same precision class at twice the tensor rate and half the bytes;
                 it is active only while cuDNN may use TF32 (torch.backends.cudnn.allow_tf32), so a strict-fp32 run stays
                 strict.  The recurrent state, the coordinates and every other conv stay fp32 (DESIGN.md §4 "Precision").
+                The generator's transformer takes fp16 operands the same way: every LayerNorm writes its output as fp16,
+                the fused QKV, pooled K/V, proj, fc1 and fc2 Linear layers run on fp16 weights and biases with fp32
+                accumulation and fp32 split-K reductions and write fp16, the depthwise pooling, the window attention (f16
+                wgmma / mma.sync kernels, fp32 softmax and accumulators) and the fold / unfold read and write fp16 rows while
+                computing in fp32, and each sublayer's fp16 output enters the fp32 residual stream in the next LayerNorm.
+                This is active only while those Linear layers would run TF32 anyway (LINEAR_TF32 or
+                torch.backends.cuda.matmul.allow_tf32, CUDA tensors), so a strict-fp32 run stays strict.
                 Environment: PP_HALF_OPERANDS=0|1.
 AUTOTUNE        time numerically equivalent plans of a step once per shape during warm-up and keep the faster
                 (propainter_b200/autotune.py): grouped conv vs per-group dense convs, conv + pp_bias_act vs cuDNN's fused
@@ -49,6 +56,22 @@ UMMA_CONV = _u if _u in ("auto", "hybrid", "hoisted") else (_u != "0")
 def half_convs():
     """whether RAFT's refinement-loop convs run on fp16 operands now (HALF_OPERANDS where cuDNN may use TF32)"""
     return bool(HALF_OPERANDS) and torch.backends.cudnn.allow_tf32
+
+
+def half_linears():
+    """whether the transformer runs on fp16 operands now (HALF_OPERANDS where its Linear layers would run TF32)"""
+    return bool(HALF_OPERANDS) and (bool(LINEAR_TF32) or torch.backends.cuda.matmul.allow_tf32)
+
+
+@contextlib.contextmanager
+def fp32_reductions():
+    """fp16 cuBLAS GEMMs with their split-K partial sums reduced in fp32 (else cuBLAS may reduce them in fp16)"""
+    prev = torch.backends.cuda.matmul.allow_fp16_reduced_precision_reduction
+    torch.backends.cuda.matmul.allow_fp16_reduced_precision_reduction = False
+    try:
+        yield
+    finally:
+        torch.backends.cuda.matmul.allow_fp16_reduced_precision_reduction = prev
 
 
 @contextlib.contextmanager

@@ -224,3 +224,206 @@ int pp_launch_sparse_attn_umma(const PPAttnParams& p, int n_windows, cudaStream_
   k_sparse_attn_umma<<<grid, UA_THREADS, UA_SMEM_BYTES, stream>>>(p);
   return cudaPeekAtLastError() == cudaSuccess ? PP_OK : PP_ERR_LAUNCH;
 }
+
+// ================================================================ fp16 operands (config.HALF_OPERANDS)
+// Same tiling and pipeline on m64nNk16 f32.f16.f16: qkv / pool rows are fp16, the output is fp16 (rounded once).  K and V
+// tiles are the same plain row copies (cp.async, no transposing producers): K is read K-major, V through the B-transpose bit
+// as an MN-major operand.  P goes from the S accumulator straight into A fragments (keys 2t, 2t+1 / 2t+8, 2t+9 of each k16
+// step are exactly the accumulator's columns of two adjacent n8 blocks).  Softmax statistics and O stay fp32.
+#define UH_BN 64
+#define UH_Q_BYTES (UA_BM * 128 * 2)               // 32 KB: 2 k-blocks of [128 rows x 128 B]
+#define UH_K_BYTES (UH_BN * 128 * 2)               // 16 KB: 2 k-blocks of [64 keys x 128 B]
+#define UH_V_BYTES (UH_BN * 128 * 2)               // 16 KB: 2 blocks of 64 head dims, [64 keys x 128 B] each (MN-major)
+#define UH_STAGE_BYTES (UH_K_BYTES + UH_V_BYTES)
+#define UH_STAGES 3
+#define UH_TAIL_BYTES 4096                         // barriers, token table (<= 224 ints at +256), key row pointers (+1152)
+#define UH_SMEM_BYTES (UH_Q_BYTES + UH_STAGES * UH_STAGE_BYTES + UH_TAIL_BYTES + 1024)
+static_assert(1152 + UH_STAGES * UH_BN * 8 <= UH_TAIL_BYTES, "key row pointers overflow the tail");
+
+__device__ __forceinline__ uint32_t uh_pack(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+__global__ void __launch_bounds__(UA_THREADS, 1) k_sparse_attn_umma_f16(PPAttnParams p) {
+  extern __shared__ __align__(1024) uint8_t ua_raw[];
+  const int win = blockIdx.z, head = blockIdx.y;
+  if (p.flags[win] == 0) return;
+  uint8_t* base = ua_raw + ((1024u - (ua_smem(ua_raw) & 1023u)) & 1023u);
+  uint8_t* sQ = base;
+  uint8_t* stages = base + UH_Q_BYTES;
+  uint8_t* tail = stages + UH_STAGES * UH_STAGE_BYTES;
+  unsigned long long* bars = reinterpret_cast<unsigned long long*>(tail);   // full[S], empty[S]
+  int* stab = reinterpret_cast<int*>(tail + 256);
+  const __half* qkv = reinterpret_cast<const __half*>(p.qkv);
+  const __half* pool = reinterpret_cast<const __half*>(p.pool);
+  __half* out = reinterpret_cast<__half*>(p.out);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int* ktab = p.key_tok + (long)win * p.NKO;
+  const int hoff = head * 128;
+  const int q0 = blockIdx.x * UA_BM;
+  const int nq = min(UA_BM, p.t * p.WN - q0);
+  const int keys_per_frame = p.NKO + p.NP;
+  const int nkeys = p.nkf * keys_per_frame;
+  const int ntiles = (nkeys + UH_BN - 1) / UH_BN;
+  const uint32_t b0 = ua_smem(&bars[0]);
+  auto bar = [&](int i) { return b0 + 8u * (uint32_t)i; };
+
+  if (tid == 0) {
+    for (int i = 0; i < UH_STAGES; ++i) { ua_bar_init(bar(i), 128); ua_bar_init(bar(UH_STAGES + i), 8); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  for (int i = tid; i < p.NKO; i += UA_THREADS) stab[i] = ktab[i];
+  __syncthreads();
+
+  if (warp >= 8) {
+    // ================================================= producers: K and V rows of the tile, both plain 16-byte copies
+    const int ptid = tid - 256;
+    for (int j = 0; j < ntiles; ++j) {
+      const int s = j % UH_STAGES, use = j / UH_STAGES;
+      ua_bar_wait(bar(UH_STAGES + s), (use & 1) ^ 1);
+      uint8_t* sK = stages + s * UH_STAGE_BYTES;
+      uint8_t* sV = sK + UH_K_BYTES;
+      const __half** kp = reinterpret_cast<const __half**>(tail + 1152) + s * UH_BN;
+      if (ptid < UH_BN) {
+        const int jk = j * UH_BN + ptid;
+        const __half* src = nullptr;
+        if (jk < nkeys) {
+          const int kfi = jk / keys_per_frame, slot = jk - kfi * keys_per_frame, fr = p.kf_start + kfi * p.kf_step;
+          src = slot < p.NKO ? qkv + ((long)fr * p.NT + stab[slot]) * p.ld_qkv + p.C + hoff
+                             : pool + ((long)fr * p.NP + (slot - p.NKO)) * p.ld_pool + hoff;
+        }
+        kp[ptid] = src;
+      }
+      asm volatile("bar.sync 1, 128;" ::: "memory");
+      // a key row is 256 bytes of K and 256 of V: 16 chunks each; chunk c8 holds head dims 8*c8 .. 8*c8+7 (4 half pairs)
+#pragma unroll 4
+      for (int i = 0; i < 8; ++i) {
+        const int kk = (ptid >> 4) + 8 * i, c8 = ptid & 15;
+        const __half* src = kp[kk];
+        const uint32_t off = ua_off(kk, c8 * 4, UH_BN);
+        if (src) {
+          pp_cp_async16(sK + off, src + c8 * 8);
+          pp_cp_async16(sV + off, src + p.C + c8 * 8);
+        } else {
+          *reinterpret_cast<uint4*>(sK + off) = make_uint4(0u, 0u, 0u, 0u);
+          *reinterpret_cast<uint4*>(sV + off) = make_uint4(0u, 0u, 0u, 0u);
+        }
+      }
+      pp_cp_async_commit();
+      pp_cp_async_wait<0>();
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      ua_bar_arrive(bar(s));
+    }
+    return;
+  }
+
+  const int wg = warp >> 2, g = lane >> 2, t = lane & 3;
+  {   // Q rows -> shared memory, scaled into the log2 domain in fp32 and rounded to fp16 once
+    const int row = wg * 64 + (tid & 63), c_half = (tid >> 6) & 1;
+    const __half* qrow = nullptr;
+    if (row < nq) { const int qi = q0 + row, fr = qi / p.WN; qrow = qkv + ((long)fr * p.NT + stab[qi - fr * p.WN]) * p.ld_qkv + hoff; }
+#pragma unroll 4
+    for (int c = c_half * 64; c < c_half * 64 + 64; c += 8) {
+      uint4 u = make_uint4(0u, 0u, 0u, 0u);
+      if (qrow) {
+        const float4 a = pp_ld4(qrow + c), b = pp_ld4(qrow + c + 4);
+        const float sc = p.scale_log2;
+        u = make_uint4(uh_pack(a.x * sc, a.y * sc), uh_pack(a.z * sc, a.w * sc), uh_pack(b.x * sc, b.y * sc), uh_pack(b.z * sc, b.w * sc));
+      }
+      *reinterpret_cast<uint4*>(sQ + ua_off(row, c / 2, UA_BM)) = u;
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    if (wg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
+    else asm volatile("bar.sync 3, 128;" ::: "memory");
+  }
+  const uint64_t qd = ua_desc(ua_smem(sQ) + (uint32_t)wg * 64 * 128);
+  float o[64], sacc[32];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  for (int j = 0; j < ntiles; ++j) {
+    const int s = j % UH_STAGES;
+    ua_bar_wait(bar(s), (j / UH_STAGES) & 1);
+    const uint32_t kaddr = ua_smem(stages + s * UH_STAGE_BYTES);
+    const uint64_t kd = ua_desc(kaddr), vd = ua_desc_mn(kaddr + UH_K_BYTES, UH_BN * 128);
+    // ---- S = Q K^T: 128 head dims = 2 k-blocks x 4 k-steps of 16
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks)
+      wg_mma_ss_n64_f16(sacc, qd + (uint64_t)(((ks >> 2) * (UA_BM * 128) + (ks & 3) * 32) >> 4),
+                        kd + (uint64_t)(((ks >> 2) * (UH_BN * 128) + (ks & 3) * 32) >> 4), ks > 0);
+    wg_commit();
+    wg_wait<0>();
+    wg_pin(sacc);
+    const int kbase = j * UH_BN;
+    if (kbase + UH_BN > nkeys) {
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        const int k0 = kbase + 8 * c + 2 * t;
+        if (k0 >= nkeys) { sacc[4 * c] = -INFINITY; sacc[4 * c + 2] = -INFINITY; }
+        if (k0 + 1 >= nkeys) { sacc[4 * c + 1] = -INFINITY; sacc[4 * c + 3] = -INFINITY; }
+      }
+    }
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      mx0 = fmaxf(mx0, fmaxf(sacc[4 * c], sacc[4 * c + 1]));
+      mx1 = fmaxf(mx1, fmaxf(sacc[4 * c + 2], sacc[4 * c + 3]));
+    }
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
+    const float al0 = exp2f(m0 - mn0), al1 = exp2f(m1 - mn1);
+    m0 = mn0; m1 = mn1;
+    float rs0 = 0.f, rs1 = 0.f;
+    float e[32];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      e[4 * c] = exp2f(sacc[4 * c] - mn0); e[4 * c + 1] = exp2f(sacc[4 * c + 1] - mn0);
+      e[4 * c + 2] = exp2f(sacc[4 * c + 2] - mn1); e[4 * c + 3] = exp2f(sacc[4 * c + 3] - mn1);
+      rs0 += e[4 * c] + e[4 * c + 1]; rs1 += e[4 * c + 2] + e[4 * c + 3];
+    }
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {                    // keys 16ks + {2t, 2t+1} = n8 block 2ks, + {8+2t, 9+2t} = block 2ks+1
+      pa[ks][0] = uh_pack(e[8 * ks], e[8 * ks + 1]);
+      pa[ks][1] = uh_pack(e[8 * ks + 2], e[8 * ks + 3]);
+      pa[ks][2] = uh_pack(e[8 * ks + 4], e[8 * ks + 5]);
+      pa[ks][3] = uh_pack(e[8 * ks + 6], e[8 * ks + 7]);
+    }
+    l0 = l0 * al0 + rs0; l1 = l1 * al1 + rs1;
+#pragma unroll
+    for (int c = 0; c < 16; ++c) { o[4 * c] *= al0; o[4 * c + 1] *= al0; o[4 * c + 2] *= al1; o[4 * c + 3] *= al1; }
+    // ---- O += P V: 64 keys = 4 k-steps of 16 = 2 swizzle atoms of 8 keys each
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) wg_mma_rs_n128_f16_tb(o, pa[ks], vd + (uint64_t)((ks * 2048) >> 4), 1);
+    wg_commit();
+    wg_wait<0>();
+    wg_pin(o);
+    if (lane == 0) ua_bar_arrive(bar(UH_STAGES + s));
+  }
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+  const int ra = wg * 64 + (warp & 3) * 16 + g, rb = ra + 8;
+  __half* oa = nullptr; __half* ob = nullptr;
+  if (ra < nq) { const int qi = q0 + ra, fr = qi / p.WN; oa = out + ((long)fr * p.NT + stab[qi - fr * p.WN]) * p.ld_out + hoff; }
+  if (rb < nq) { const int qi = q0 + rb, fr = qi / p.WN; ob = out + ((long)fr * p.NT + stab[qi - fr * p.WN]) * p.ld_out + hoff; }
+#pragma unroll
+  for (int c = 0; c < 16; ++c) {
+    const int n = 8 * c + 2 * t;
+    if (oa) *reinterpret_cast<uint32_t*>(oa + n) = uh_pack(o[4 * c] * inv0, o[4 * c + 1] * inv0);
+    if (ob) *reinterpret_cast<uint32_t*>(ob + n) = uh_pack(o[4 * c + 2] * inv1, o[4 * c + 3] * inv1);
+  }
+}
+
+int pp_launch_sparse_attn_umma_f16(const PPAttnParams& p, int n_windows, cudaStream_t stream) {
+  if (p.NKO > 224) return PP_ERR_SHAPE;
+  if (cudaFuncSetAttribute(k_sparse_attn_umma_f16, cudaFuncAttributeMaxDynamicSharedMemorySize, UH_SMEM_BYTES) != cudaSuccess)
+    return PP_ERR_LAUNCH;
+  dim3 grid((p.t * p.WN + UA_BM - 1) / UA_BM, p.C / 128, n_windows);
+  k_sparse_attn_umma_f16<<<grid, UA_THREADS, UH_SMEM_BYTES, stream>>>(p);
+  return cudaPeekAtLastError() == cudaSuccess ? PP_OK : PP_ERR_LAUNCH;
+}

@@ -338,20 +338,23 @@ extern "C" int pp_window_mask(const float* pmask, int lt, int h, int w, int fh, 
 
 // ================================================================ fusion feed-forward overlap-add
 // fold (+ /count + GELU, applied once per feature pixel instead of once per (token, tap)) ...
-__global__ void __launch_bounds__(256) k_ffn_fold_gelu(const float* __restrict__ Y, int ldy, int CH, int fh, int fw, int h,
+// T = __half (the transformer's half-operand Linear layers): fc1's fp16 output in, fc2's fp16 operand out; the fold sums in
+// fp32 in the same order and the workspace F stays fp32, so the result is the fp32 kernel's on the widened rows, rounded once.
+template <typename T>
+__global__ void __launch_bounds__(256) k_ffn_fold_gelu(const T* __restrict__ Y, int ldy, int CH, int fh, int fw, int h,
                                                        int w, float* __restrict__ F) {
   const int c4n = CH >> 2;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;       // over h*w*(CH/4) of frame blockIdx.y
   if (i >= h * w * c4n) return;
   const int c = (i % c4n) * 4, px = i / c4n, y = px / w, x = px - y * w;
-  const float* Yf = Y + (long)blockIdx.y * fh * fw * ldy;
+  const T* Yf = Y + (long)blockIdx.y * fh * fw * ldy;
   float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
   int n = 0;
   for (int ty = (y + 3) / 3, ky; ty >= 0 && (ky = y + 3 - 3 * ty) < 7; --ty) {
     if (ty >= fh) continue;
     for (int tx = (x + 3) / 3, kx; tx >= 0 && (kx = x + 3 - 3 * tx) < 7; --tx) {
       if (tx >= fw) continue;
-      const float4 v = *reinterpret_cast<const float4*>(Yf + (long)(ty * fw + tx) * ldy + (ky * 7 + kx) * CH + c);
+      const float4 v = pp_ld4(Yf + (long)(ty * fw + tx) * ldy + (ky * 7 + kx) * CH + c);
       s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
       ++n;
     }
@@ -362,8 +365,9 @@ __global__ void __launch_bounds__(256) k_ffn_fold_gelu(const float* __restrict__
   *reinterpret_cast<float4*>(F + ((long)blockIdx.y * h * w + px) * CH + c) = o;
 }
 // ... then unfold is a pure gather-copy (out-of-image taps read as gelu(0) = 0)
+template <typename T>
 __global__ void __launch_bounds__(256) k_ffn_unfold(const float* __restrict__ F, int CH, int fh, int fw, int h, int w,
-                                                    float* __restrict__ Z, int ldz) {
+                                                    T* __restrict__ Z, int ldz) {
   const int c4n = CH >> 2;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;       // over fh*fw*49*(CH/4) of frame blockIdx.y
   if (i >= fh * fw * 49 * c4n) return;
@@ -372,27 +376,40 @@ __global__ void __launch_bounds__(256) k_ffn_unfold(const float* __restrict__ F,
   float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
   if (y >= 0 && y < h && x >= 0 && x < w)
     v = *reinterpret_cast<const float4*>(F + (((long)blockIdx.y * h + y) * w + x) * CH + c);
-  *reinterpret_cast<float4*>(Z + ((long)blockIdx.y * fh * fw + tok) * ldz + tap * CH + c) = v;
+  pp_st4(Z + ((long)blockIdx.y * fh * fw + tok) * ldz + tap * CH + c, v);
 }
 
 extern "C" size_t pp_ffn_overlap_add_workspace_bytes(int frames, int h, int w, int CH) {
   return (size_t)frames * h * w * CH * sizeof(float);
 }
-// replaces fold -> /normalizer -> unfold -> GELU of FusionFeedForward.forward
-// (model/modules/sparse_transformer.py:81-100).  Y,Z: [frames*fh*fw][ld], columns tap-major (tap*CH+c).
-extern "C" int pp_ffn_overlap_add(const float* Y, int ldy, float* Z, int ldz, int frames, int h, int w, int CH,
-                                  void* workspace, size_t ws_bytes, cudaStream_t stream) {
+template <typename T>
+static int pp_ffn_launch(const T* Y, int ldy, T* Z, int ldz, int frames, int h, int w, int CH, void* workspace, size_t ws_bytes,
+                         cudaStream_t stream) {
   const int fh = (h - 1) / 3 + 1, fw = (w - 1) / 3 + 1;
-  if (ldy < 49 * CH || ldz < 49 * CH || frames < 1 || frames > 65535) return PP_ERR_SHAPE;
-  if (CH % 4 || ldy % 4 || ldz % 4) return PP_ERR_ALIGN;
   if (ws_bytes < pp_ffn_overlap_add_workspace_bytes(frames, h, w, CH)) return PP_ERR_WORKSPACE;
   float* F = (float*)workspace;
   const long n1 = (long)h * w * (CH / 4), n2 = (long)fh * fw * 49 * (CH / 4);
   if (n2 > 0x7fffffffL) return PP_ERR_SHAPE;
-  k_ffn_fold_gelu<<<dim3(pp_blocks(n1, 256), frames), 256, 0, stream>>>(Y, ldy, CH, fh, fw, h, w, F);
-  k_ffn_unfold<<<dim3(pp_blocks(n2, 256), frames), 256, 0, stream>>>(F, CH, fh, fw, h, w, Z, ldz);
+  k_ffn_fold_gelu<T><<<dim3(pp_blocks(n1, 256), frames), 256, 0, stream>>>(Y, ldy, CH, fh, fw, h, w, F);
+  k_ffn_unfold<T><<<dim3(pp_blocks(n2, 256), frames), 256, 0, stream>>>(F, CH, fh, fw, h, w, Z, ldz);
   PP_LAUNCH_CHECK();
   return PP_OK;
+}
+// replaces fold -> /normalizer -> unfold -> GELU of FusionFeedForward.forward
+// (model/modules/sparse_transformer.py:81-100).  Y,Z: [frames*fh*fw][ld], columns tap-major (tap*CH+c).
+extern "C" int pp_ffn_overlap_add(const float* Y, int ldy, float* Z, int ldz, int frames, int h, int w, int CH,
+                                  void* workspace, size_t ws_bytes, cudaStream_t stream) {
+  if (ldy < 49 * CH || ldz < 49 * CH || frames < 1 || frames > 65535) return PP_ERR_SHAPE;
+  if (CH % 4 || ldy % 4 || ldz % 4) return PP_ERR_ALIGN;
+  return pp_ffn_launch(Y, ldy, Z, ldz, frames, h, w, CH, workspace, ws_bytes, stream);
+}
+// the same on fp16 rows of Y and Z (16-byte aligned, ld % 8 == 0); frames = 0 returns PP_OK without a launch
+extern "C" int pp_ffn_overlap_add_f16(const void* Y, int ldy, void* Z, int ldz, int frames, int h, int w, int CH,
+                                      void* workspace, size_t ws_bytes, cudaStream_t stream) {
+  if (ldy < 49 * CH || ldz < 49 * CH || frames < 0 || frames > 65535) return PP_ERR_SHAPE;
+  if (CH % 4 || ldy % 8 || ldz % 8 || ((uintptr_t)Y & 15) || ((uintptr_t)Z & 15) || ((uintptr_t)workspace & 15)) return PP_ERR_ALIGN;
+  if (frames == 0 || h <= 0 || w <= 0) return PP_OK;
+  return pp_ffn_launch((const __half*)Y, ldy, (__half*)Z, ldz, frames, h, w, CH, workspace, ws_bytes, stream);
 }
 
 // ================================================================ conv epilogue + x2 upsampling
@@ -824,8 +841,11 @@ extern "C" int pp_upflow8(const float* flow_lr, float* out, int n, int h, int w,
 // ================================================================ transformer glue
 // pool_layer of SparseWindowAttention (sparse_transformer.py:131-133,203-206): depthwise Conv2d with kernel = stride =
 // pool_size, no padding, on the pixel-major token grid.  x [n][H][W][C] (pixel stride ld_x), w tap-major [kh*kw][C].
-__global__ void __launch_bounds__(256) k_pool_depthwise(const float* __restrict__ x, int ld_x, const float* __restrict__ w,
-    const float* __restrict__ bias, float* __restrict__ out, int n, int H, int W, int C, int kh, int kw, int ph, int pw) {
+// T = __half: the fp16 LayerNorm output in, fp16 pooled tokens out (the operand of the pooled K/V Linear); weights, bias and
+// the fma chain stay fp32, rounded once on the store.
+template <typename T>
+__global__ void __launch_bounds__(256) k_pool_depthwise(const T* __restrict__ x, int ld_x, const float* __restrict__ w,
+    const float* __restrict__ bias, T* __restrict__ out, int n, int H, int W, int C, int kh, int kw, int ph, int pw) {
   const int c4n = C >> 2;
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long)n * ph * pw * c4n) return;
@@ -834,11 +854,11 @@ __global__ void __launch_bounds__(256) k_pool_depthwise(const float* __restrict_
   float4 acc = *reinterpret_cast<const float4*>(bias + c);
   for (int a = 0; a < kh; ++a)
     for (int b = 0; b < kw; ++b) {
-      const float4 v = *reinterpret_cast<const float4*>(x + (((long)f * H + (py * kh + a)) * W + (px * kw + b)) * ld_x + c);
+      const float4 v = pp_ld4(x + (((long)f * H + (py * kh + a)) * W + (px * kw + b)) * ld_x + c);
       const float4 k = *reinterpret_cast<const float4*>(w + (long)(a * kw + b) * C + c);
       acc.x = fmaf(v.x, k.x, acc.x); acc.y = fmaf(v.y, k.y, acc.y); acc.z = fmaf(v.z, k.z, acc.z); acc.w = fmaf(v.w, k.w, acc.w);
     }
-  *reinterpret_cast<float4*>(out + i * 4) = acc;
+  pp_st4(out + i * 4, acc);
 }
 extern "C" int pp_pool_depthwise(const float* x, int ld_x, const float* w_taps, const float* bias, float* out, int n, int H, int W,
                                  int C, int kh, int kw, cudaStream_t stream) {
@@ -847,7 +867,22 @@ extern "C" int pp_pool_depthwise(const float* x, int ld_x, const float* w_taps, 
   if (kh < 1 || kw < 1 || H < kh || W < kw || n < 1 || ld_x < C) return PP_ERR_SHAPE;
   const int ph = (H - kh) / kh + 1, pw = (W - kw) / kw + 1;
   const long total = (long)n * ph * pw * (C / 4);
-  k_pool_depthwise<<<pp_blocks(total, 256), 256, 0, stream>>>(x, ld_x, w_taps, bias, out, n, H, W, C, kh, kw, ph, pw);
+  k_pool_depthwise<float><<<pp_blocks(total, 256), 256, 0, stream>>>(x, ld_x, w_taps, bias, out, n, H, W, C, kh, kw, ph, pw);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+// the same on fp16 x and out (16-byte aligned, C % 8 == 0, ld_x % 8 == 0); n = 0 returns PP_OK without a launch
+extern "C" int pp_pool_depthwise_f16(const void* x, int ld_x, const float* w_taps, const float* bias, void* out, int n, int H, int W,
+                                     int C, int kh, int kw, cudaStream_t stream) {
+  if (C % 8 || ld_x % 8 || ((uintptr_t)x & 15) || ((uintptr_t)w_taps & 15) || ((uintptr_t)bias & 15) || ((uintptr_t)out & 15))
+    return PP_ERR_ALIGN;
+  if (kh < 1 || kw < 1 || n < 0 || ld_x < C) return PP_ERR_SHAPE;
+  if (n == 0) return PP_OK;
+  if (H < kh || W < kw) return PP_ERR_SHAPE;
+  const int ph = (H - kh) / kh + 1, pw = (W - kw) / kw + 1;
+  const long total = (long)n * ph * pw * (C / 4);
+  k_pool_depthwise<__half><<<pp_blocks(total, 256), 256, 0, stream>>>((const __half*)x, ld_x, w_taps, bias, (__half*)out, n, H, W, C,
+                                                                     kh, kw, ph, pw);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }
@@ -855,9 +890,11 @@ extern "C" int pp_pool_depthwise(const float* x, int ld_x, const float* w_taps, 
 // residual add + LayerNorm of TemporalSparseTransformer.forward (sparse_transformer.py:322-334): x_out = x + delta,
 // y = LN(x_out)*gamma + beta in one pass (one warp per token row, statistics two-pass in registers).  delta == NULL:
 // plain LayerNorm (x_out not written).
-template <int NV>
-__global__ void __launch_bounds__(256) k_add_layernorm(const float* __restrict__ x, const float* __restrict__ delta,
-    const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ x_out, float* __restrict__ y, long rows,
+// TD / TY = __half: fp16 delta (fc2's fp16 output) and / or fp16 y (the operand of the next half-operand Linear layers); the
+// residual stream x / x_out, the statistics and the arithmetic stay fp32, y is rounded once on the store.
+template <int NV, typename TD, typename TY>
+__global__ void __launch_bounds__(256) k_add_layernorm(const float* __restrict__ x, const TD* __restrict__ delta,
+    const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ x_out, TY* __restrict__ y, long rows,
     float eps) {
   constexpr int C = NV * 128;
   const long row = (long)blockIdx.x * 8 + (threadIdx.x >> 5);
@@ -870,7 +907,7 @@ __global__ void __launch_bounds__(256) k_add_layernorm(const float* __restrict__
     const long off = row * C + (k * 32 + lane) * 4;
     v[k] = *reinterpret_cast<const float4*>(x + off);
     if (delta != nullptr) {
-      const float4 d = *reinterpret_cast<const float4*>(delta + off);
+      const float4 d = pp_ld4(delta + off);
       v[k].x += d.x; v[k].y += d.y; v[k].z += d.z; v[k].w += d.w;
       *reinterpret_cast<float4*>(x_out + off) = v[k];
     }
@@ -895,25 +932,38 @@ __global__ void __launch_bounds__(256) k_add_layernorm(const float* __restrict__
     float4 o;
     o.x = (v[k].x - mean) * rstd * g.x + b.x; o.y = (v[k].y - mean) * rstd * g.y + b.y;
     o.z = (v[k].z - mean) * rstd * g.z + b.z; o.w = (v[k].w - mean) * rstd * g.w + b.w;
-    *reinterpret_cast<float4*>(y + row * C + ci) = o;
+    pp_st4(y + row * C + ci, o);
   }
 }
-extern "C" int pp_add_layernorm(const float* x, const float* delta, const float* gamma, const float* beta, float* x_out, float* y,
-                                long rows, int C, float eps, cudaStream_t stream) {
-  if (((uintptr_t)x & 15) || ((uintptr_t)delta & 15) || ((uintptr_t)gamma & 15) || ((uintptr_t)beta & 15) ||
-      ((uintptr_t)x_out & 15) || ((uintptr_t)y & 15)) return PP_ERR_ALIGN;
-  if (rows < 0 || (delta != nullptr && x_out == nullptr)) return PP_ERR_SHAPE;
-  if (rows == 0) return PP_OK;
+template <typename TD, typename TY>
+static int pp_add_layernorm_launch(const float* x, const TD* delta, const float* gamma, const float* beta, float* x_out, TY* y,
+                                   long rows, int C, float eps, cudaStream_t stream) {
   const unsigned grid = (unsigned)((rows + 7) / 8);
   switch (C) {
-    case 128: k_add_layernorm<1><<<grid, 256, 0, stream>>>(x, delta, gamma, beta, x_out, y, rows, eps); break;
-    case 256: k_add_layernorm<2><<<grid, 256, 0, stream>>>(x, delta, gamma, beta, x_out, y, rows, eps); break;
-    case 512: k_add_layernorm<4><<<grid, 256, 0, stream>>>(x, delta, gamma, beta, x_out, y, rows, eps); break;
-    case 1024: k_add_layernorm<8><<<grid, 256, 0, stream>>>(x, delta, gamma, beta, x_out, y, rows, eps); break;
+    case 128: k_add_layernorm<1, TD, TY><<<grid, 256, 0, stream>>>(x, delta, gamma, beta, x_out, y, rows, eps); break;
+    case 256: k_add_layernorm<2, TD, TY><<<grid, 256, 0, stream>>>(x, delta, gamma, beta, x_out, y, rows, eps); break;
+    case 512: k_add_layernorm<4, TD, TY><<<grid, 256, 0, stream>>>(x, delta, gamma, beta, x_out, y, rows, eps); break;
+    case 1024: k_add_layernorm<8, TD, TY><<<grid, 256, 0, stream>>>(x, delta, gamma, beta, x_out, y, rows, eps); break;
     default: return PP_ERR_SHAPE;
   }
   PP_LAUNCH_CHECK();
   return PP_OK;
+}
+// the same with fp16 (delta_f16 != 0) or fp32 delta and fp16 (y_f16 != 0) or fp32 y; x / x_out stay fp32
+extern "C" int pp_add_layernorm_f16(const float* x, const void* delta, int delta_f16, const float* gamma, const float* beta,
+                                    float* x_out, void* y, int y_f16, long rows, int C, float eps, cudaStream_t stream) {
+  if (((uintptr_t)x & 15) || ((uintptr_t)delta & 15) || ((uintptr_t)gamma & 15) || ((uintptr_t)beta & 15) ||
+      ((uintptr_t)x_out & 15) || ((uintptr_t)y & 15)) return PP_ERR_ALIGN;
+  if (rows < 0 || (delta != nullptr && x_out == nullptr)) return PP_ERR_SHAPE;
+  if (rows == 0) return PP_OK;
+  if (delta_f16 && y_f16) return pp_add_layernorm_launch(x, (const __half*)delta, gamma, beta, x_out, (__half*)y, rows, C, eps, stream);
+  if (delta_f16) return pp_add_layernorm_launch(x, (const __half*)delta, gamma, beta, x_out, (float*)y, rows, C, eps, stream);
+  if (y_f16) return pp_add_layernorm_launch(x, (const float*)delta, gamma, beta, x_out, (__half*)y, rows, C, eps, stream);
+  return pp_add_layernorm_launch(x, (const float*)delta, gamma, beta, x_out, (float*)y, rows, C, eps, stream);
+}
+extern "C" int pp_add_layernorm(const float* x, const float* delta, const float* gamma, const float* beta, float* x_out, float* y,
+                                long rows, int C, float eps, cudaStream_t stream) {
+  return pp_add_layernorm_f16(x, delta, 0, gamma, beta, x_out, y, 0, rows, C, eps, stream);
 }
 
 // ================================================================ mask preparation

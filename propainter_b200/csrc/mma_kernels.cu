@@ -2,6 +2,7 @@
 //   * pp_corr_build        RAFT all-pairs correlation (3xTF32 split => fp32-accurate), level-0 writer
 //   * pp_deform_align      modulated deformable 3x3 alignment: offset prep + bilinear gather + GEMM fused
 //   * pp_sparse_window_attn mask-guided sparse window attention, flash-style, K/V gathered arithmetically
+//   * pp_sparse_window_attn_f16 the same on fp16 operands (unmasked windows here on m16n8k16, masked ones in attn_umma.cu)
 #include "pp_elem.cuh"
 #include "pp_mma.cuh"
 #include "../../include/propainter_b200.h"
@@ -524,7 +525,136 @@ __global__ void __launch_bounds__(128, 2) k_attn_unmasked_frames(PPAttnParams p,
   }
 }
 
+// fp16 operands (config.HALF_OPERANDS): the unmasked-window kernel above on mma.sync m16n8k16 f32.f16.f16.  fp16 qkv rows in,
+// fp16 out (rounded once); Q scaled into the log2 domain in fp32 and rounded once; P's accumulator fragment is the A fragment
+// of the P V step as it stands, V fragments come transposed out of row-major key rows by ldmatrix.trans.
+#define AH_LD 136                                 // halves per staged key row: 272 bytes, conflict-free ldmatrix / 32-bit loads
+#define AH_STAGE (2 * AU_KEYS * AH_LD)
+__device__ __forceinline__ uint32_t ah_pack(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+__global__ void __launch_bounds__(128, 2) k_attn_unmasked_frames_f16(PPAttnParams p, int fpc) {
+  extern __shared__ __align__(16) __half hsm[];
+  const int win = blockIdx.z, head = blockIdx.y;
+  if (p.flags[win] != 0) return;
+  const __half* qkv = reinterpret_cast<const __half*>(p.qkv);
+  __half* out = reinterpret_cast<__half*>(p.out);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const int* ktab = p.key_tok + (long)win * p.NKO;
+  const int hoff = head * 128, WN = p.WN;
+  const int f0 = blockIdx.x * fpc, f1 = min(p.t, f0 + fpc);
+  if (f0 >= f1) return;
+  auto Kst = [&](int st) { return hsm + st * AH_STAGE; };
+  auto Vst = [&](int st) { return hsm + st * AH_STAGE + AU_KEYS * AH_LD; };
+  auto gather = [&](int f, int st) {
+    __half* Ks = Kst(st); __half* Vs = Vst(st);
+    for (int idx = tid; idx < WN * 16; idx += 128) {
+      const int key = idx >> 4, c8 = idx & 15;
+      const __half* src = qkv + ((long)f * p.NT + ktab[key]) * p.ld_qkv + p.C + hoff;
+      pp_cp_async16(Ks + key * AH_LD + c8 * 8, src + c8 * 8);
+      pp_cp_async16(Vs + key * AH_LD + c8 * 8, src + p.C + c8 * 8);
+    }
+    pp_cp_async_commit();
+  };
+  // pad key rows [WN, 48) of both stages: zero once (their P is 0, but 0 * stale-NaN would poison the accumulators)
+  for (int idx = tid; idx < 2 * (AU_KEYS - WN) * 16; idx += 128) {
+    const int st = idx / ((AU_KEYS - WN) * 16), r = idx - st * (AU_KEYS - WN) * 16, key = WN + (r >> 4), c8 = r & 15;
+    *reinterpret_cast<uint4*>(Kst(st) + key * AH_LD + c8 * 8) = make_uint4(0u, 0u, 0u, 0u);
+    *reinterpret_cast<uint4*>(Vst(st) + key * AH_LD + c8 * 8) = make_uint4(0u, 0u, 0u, 0u);
+  }
+  gather(f0, 0);
+  const int ra = warp * 16 + g, rb = ra + 8;
+  const int ta = ra < WN ? ktab[ra] : -1, tb = rb < WN ? ktab[rb] : -1;
+  for (int f = f0; f < f1; ++f) {
+    const int cur = (f - f0) & 1;
+    uint32_t qa[8][4];
+    {
+      const __half* r0 = qkv + ((long)f * p.NT + (ta >= 0 ? ta : 0)) * p.ld_qkv + hoff;
+      const __half* r1 = qkv + ((long)f * p.NT + (tb >= 0 ? tb : 0)) * p.ld_qkv + hoff;
+      const float sc = p.scale_log2;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int d = 16 * j + 8 * h + 2 * t;
+          float2 lo = make_float2(0.f, 0.f), hi = lo;
+          if (ta >= 0) lo = __half22float2(*reinterpret_cast<const __half2*>(r0 + d));
+          if (tb >= 0) hi = __half22float2(*reinterpret_cast<const __half2*>(r1 + d));
+          qa[j][2 * h] = ah_pack(lo.x * sc, lo.y * sc);
+          qa[j][2 * h + 1] = ah_pack(hi.x * sc, hi.y * sc);
+        }
+      }
+    }
+    pp_cp_async_wait<0>();
+    __syncthreads();
+    if (f + 1 < f1) gather(f + 1, cur ^ 1);
+    if (warp * 16 >= WN) continue;
+    const __half* Ks = Kst(cur); const __half* Vs = Vst(cur);
+    float s[6][4];
+#pragma unroll
+    for (int nt = 0; nt < 6; ++nt) {
+      s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
+      const __half* kr = Ks + (nt * 8 + g) * AH_LD + 2 * t;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const uint32_t b[2] = {*reinterpret_cast<const uint32_t*>(kr + 16 * j), *reinterpret_cast<const uint32_t*>(kr + 16 * j + 8)};
+        pp_mma_f16(s[nt], qa[j], b);
+      }
+    }
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int nt = 0; nt < 6; ++nt) {
+      const int j = nt * 8 + 2 * t;
+      if (j >= WN) { s[nt][0] = -INFINITY; s[nt][2] = -INFINITY; }
+      if (j + 1 >= WN) { s[nt][1] = -INFINITY; s[nt][3] = -INFINITY; }
+      mx0 = fmaxf(mx0, fmaxf(s[nt][0], s[nt][1]));
+      mx1 = fmaxf(mx1, fmaxf(s[nt][2], s[nt][3]));
+    }
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    float l0 = 0.f, l1 = 0.f;
+#pragma unroll
+    for (int nt = 0; nt < 6; ++nt) {
+      s[nt][0] = exp2f(s[nt][0] - mx0); s[nt][1] = exp2f(s[nt][1] - mx0);
+      s[nt][2] = exp2f(s[nt][2] - mx1); s[nt][3] = exp2f(s[nt][3] - mx1);
+      l0 += s[nt][0] + s[nt][1]; l1 += s[nt][2] + s[nt][3];
+    }
+    float oacc[16][4];
+#pragma unroll
+    for (int a = 0; a < 16; ++a)
+#pragma unroll
+      for (int b = 0; b < 4; ++b) oacc[a][b] = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < 3; ++kk) {                       // 16 keys per step: n8 blocks 2kk (keys 2t..) and 2kk+1 (keys 8+2t..)
+      const uint32_t a[4] = {ah_pack(s[2 * kk][0], s[2 * kk][1]), ah_pack(s[2 * kk][2], s[2 * kk][3]),
+                             ah_pack(s[2 * kk + 1][0], s[2 * kk + 1][1]), ah_pack(s[2 * kk + 1][2], s[2 * kk + 1][3])};
+      const __half* vrow = Vs + (16 * kk + ((lane >> 3) & 1) * 8 + (lane & 7)) * AH_LD + (lane >> 4) * 8;
+#pragma unroll
+      for (int np = 0; np < 8; ++np) {                     // head dims 16np .. 16np+15 = n8 tiles 2np, 2np+1
+        uint32_t r[4];
+        pp_ldmatrix_x4_trans(r, vrow + 16 * np);
+        const uint32_t b0[2] = {r[0], r[1]}, b1[2] = {r[2], r[3]};
+        pp_mma_f16(oacc[2 * np], a, b0);
+        pp_mma_f16(oacc[2 * np + 1], a, b1);
+      }
+    }
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+    __half* oa = ta >= 0 ? out + ((long)f * p.NT + ta) * p.ld_out + hoff : nullptr;
+    __half* ob = tb >= 0 ? out + ((long)f * p.NT + tb) * p.ld_out + hoff : nullptr;
+#pragma unroll
+    for (int nt = 0; nt < 16; ++nt) {
+      const int n = 8 * nt + 2 * t;
+      if (oa) *reinterpret_cast<uint32_t*>(oa + n) = ah_pack(oacc[nt][0] * inv0, oacc[nt][1] * inv0);
+      if (ob) *reinterpret_cast<uint32_t*>(ob + n) = ah_pack(oacc[nt][2] * inv1, oacc[nt][3] * inv1);
+    }
+  }
+}
+
 int pp_launch_sparse_attn_umma(const PPAttnParams& p, int n_windows, cudaStream_t stream);   // attn_umma.cu
+int pp_launch_sparse_attn_umma_f16(const PPAttnParams& p, int n_windows, cudaStream_t stream);
 
 static int pp_attn_check(const PPAttnParams& p) {
   if (p.C != 512 || p.WN > 64 || p.WN < 1 || p.ld_qkv % 4 || p.ld_pool % 4 || p.ld_out % 4 || p.nkf < 0) return PP_ERR_SHAPE;
@@ -583,4 +713,27 @@ extern "C" int pp_sparse_window_attn_mma(const PPAttnParams* prm, int n_windows,
   k_sparse_attn<true, 8><<<gm, 256, smem, stream>>>(p);
   PP_LAUNCH_CHECK();
   return pp_attn_unmasked(p, n_windows, stream);
+}
+
+// fp16 qkv / pool_kv in, fp16 out: masked windows on the f16 wgmma kernel (attn_umma.cu), unmasked windows on the f16 mma.sync
+// kernel above.  Rows 16-byte aligned with ld % 8 == 0 (else PP_ERR_ALIGN); t = 0 or no window returns PP_OK without a launch.
+extern "C" int pp_sparse_window_attn_f16(const PPAttnParams* prm, int n_windows, cudaStream_t stream) {
+  const PPAttnParams& p = *prm;
+  if (p.C != 512 || p.WN > AU_KEYS || p.WN < 1 || p.nkf < 0 || p.t < 0 || n_windows < 0) return PP_ERR_SHAPE;
+  if (p.ld_qkv % 8 || p.ld_pool % 8 || p.ld_out % 8 || ((uintptr_t)p.qkv & 15) || ((uintptr_t)p.pool & 15) || ((uintptr_t)p.out & 15))
+    return PP_ERR_ALIGN;
+  if (p.t == 0 || n_windows == 0) return PP_OK;
+  if (p.nkf > 0) {                                         // nkf == 0: see pp_sparse_window_attn (the caller pre-zeroes `out`)
+    const int rc = pp_launch_sparse_attn_umma_f16(p, n_windows, stream);
+    if (rc != PP_OK) return rc;
+  }
+  const int smem = 2 * AH_STAGE * (int)sizeof(__half);
+  if (cudaFuncSetAttribute(k_attn_unmasked_frames_f16, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
+    return PP_ERR_LAUNCH;
+  int fpc = (p.t * (p.C / 128) * n_windows + 2 * PP_NUM_SMS - 1) / (2 * PP_NUM_SMS);
+  fpc = fpc < 1 ? 1 : (fpc > 8 ? 8 : fpc);
+  dim3 gl((p.t + fpc - 1) / fpc, p.C / 128, n_windows);
+  k_attn_unmasked_frames_f16<<<gl, 128, smem, stream>>>(p, fpc);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
 }

@@ -19,6 +19,19 @@ __device__ __forceinline__ void pp_mma_tf32(float (&d)[4], const uint32_t (&a)[4
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
+// D += A(16x16, f16, row) * B(16x8, f16, col), fp32 accumulate: a = rows g / g+8 x k 2t..2t+1 / 2t+8..2t+9, b = k 2t..2t+1 /
+// 2t+8..2t+9 x n g, packed half2
+__device__ __forceinline__ void pp_mma_f16(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+// four transposed 8x8 b16 matrices; lane l supplies the address of row l % 8 of matrix l / 8
+__device__ __forceinline__ void pp_ldmatrix_x4_trans(uint32_t (&r)[4], const void* smem_row) {
+  const uint32_t a = (uint32_t)__cvta_generic_to_shared(smem_row);
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
+}
 __device__ __forceinline__ void pp_cp_async16(void* smem, const void* gmem) {
   uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(s), "l"(gmem));

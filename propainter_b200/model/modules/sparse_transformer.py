@@ -70,6 +70,18 @@ class TransformerExec:
                     P[p + "fc2.1.weight"][:, perm].contiguous(), P[p + "fc2.1.bias"].contiguous())
         return self.net.packed(f"ffn{i}", build)
 
+    def _qkv_half(self, i):
+        """fp16 copies of the fused QKV and pooled K/V weights and biases; the depthwise pooling weights stay fp32"""
+        return self.net.packed(f"f16:qkv{i}", lambda: tuple(t.half() for t in self._qkv(i)[:4]) + self._qkv(i)[4:])
+
+    def _proj_half(self, i):
+        P, p = self.net.P, f"transformers.transformer.{i}.attention.proj."
+        return self.net.packed(f"f16:proj{i}", lambda: (P[p + "weight"].half(), P[p + "bias"].half()))
+
+    def _ffn_half(self, i):
+        """fp16 copies of fc1 / fc2 weights and biases"""
+        return self.net.packed(f"f16:ffn{i}", lambda: tuple(t.half() for t in self._ffn(i)))
+
     # ------------------------------------------------------------------ soft split / composition
     def soft_split(self, feat):
         """feat [t,c,h,w] channels_last -> tokens [t,fh,fw,hidden] pixel-major (SoftSplit.forward :19-31)."""
@@ -90,9 +102,12 @@ class TransformerExec:
         """tokens [t,fh,fw,C]; flags int32 [n_windows] (1 = masked window).  :294-344."""
         assert self.depths % t_dilation == 0, "wrong t_dilation input."
         with config.linear_precision():
-            return self._run(tokens, hw, flags, t_dilation)
+            if tokens.is_cuda and config.half_linears():              # cuBLAS only: elsewhere there is no TF32
+                with config.fp32_reductions():
+                    return self._run(tokens, hw, flags, t_dilation, True)
+            return self._run(tokens, hw, flags, t_dilation, False)
 
-    def _run(self, tokens, hw, flags, t_dilation):
+    def _run(self, tokens, hw, flags, t_dilation, half):
         t, fh, fw, C = tokens.shape
         H2, W2 = padded_grid(fh, fw, WIN)
         NT = H2 * W2
@@ -101,10 +116,12 @@ class TransformerExec:
         x = tokens.contiguous()
         pad = (H2 != fh) or (W2 != fw)
         norm = lambda i, k: (P[f"transformers.transformer.{i}.norm{k}.weight"], P[f"transformers.transformer.{i}.norm{k}.bias"])
-        _, y = ops.add_layernorm(x, None, *norm(0, 1))
+        yd = {"y_dtype": torch.float16} if half else {}                # half: every LayerNorm output is a GEMM operand
+        _, y = ops.add_layernorm(x, None, *norm(0, 1), **yd)
         for i in range(self.depths):
             p = f"transformers.transformer.{i}."
-            wqkv, bqkv, wkv, bkv, wpool, bpool = self._qkv(i)
+            wqkv, bqkv, wkv, bkv, wpool, bpool = self._qkv_half(i) if half else self._qkv(i)
+            wproj, bproj = self._proj_half(i) if half else (P[p + "attention.proj.weight"], P[p + "attention.proj.bias"])
             if pad:                                                    # zeros are padded *before* q/k/v (:168-176)
                 y = F.pad(y, (0, 0, 0, W2 - fw, 0, H2 - fh))
             qkv = F.linear(y, wqkv, bqkv).view(t, NT, 3 * C)
@@ -115,13 +132,13 @@ class TransformerExec:
             if pad:
                 att = att[:, :fh, :fw]
             # x = x + proj(att); y = norm2(x)   (residual add fused into the LayerNorm pass)
-            x, y = ops.add_layernorm(x, F.linear(att, P[p + "attention.proj.weight"], P[p + "attention.proj.bias"]), *norm(i, 2))
-            w1, b1, w2, b2 = self._ffn(i)
+            x, y = ops.add_layernorm(x, F.linear(att, wproj, bproj), *norm(i, 2), **yd)
+            w1, b1, w2, b2 = self._ffn_half(i) if half else self._ffn(i)
             hdn = F.linear(y.reshape(t * fh * fw, C), w1, b1)
             hdn = ops.ffn_overlap_add(hdn, t, hw[0], hw[1], self.ffn_ch)
             d = F.linear(hdn, w2, b2).view(t, fh, fw, C)
             if i + 1 < self.depths:                                    # x = x + mlp(y); y = norm1 of the next block
-                x, y = ops.add_layernorm(x, d, *norm(i + 1, 1))
+                x, y = ops.add_layernorm(x, d, *norm(i + 1, 1), **yd)
             else:
-                x = x + d
+                x = x + d                                              # fp16 d is widened exactly
         return x

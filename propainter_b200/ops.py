@@ -1,6 +1,7 @@
 """Tensor-level wrappers over the C ABI.  Each takes/returns torch CUDA tensors, passes raw pointers +
 the current stream, and raises on any non-zero return code.  fp32, except the fp16 operand / result tensors of RAFT's
-half-precision refinement convs (corr_lookup, bias_act, gru_gate, gru_update, raft_pack_motion; DESIGN.md §4 "Precision")."""
+half-precision refinement convs (corr_lookup, bias_act, gru_gate, gru_update, raft_pack_motion) and of the transformer's
+half-operand transformer (sparse_window_attn, pool_depthwise, ffn_overlap_add, add_layernorm); DESIGN.md §4 "Precision"."""
 import collections
 import ctypes
 import math
@@ -392,9 +393,11 @@ def window_mask(pmask, fh, fw, nwh, nww):
 
 def sparse_window_attn(qkv, pool_kv, key_tok, flags, t, NT, kf_start, kf_step, out=None, WN=45, C=512, impl="umma"):
     """qkv [t,NT,3C]; pool_kv [t,NP,2C]; key_tok int32 [nwin,NKO]; flags int32 [nwin] -> out [t,NT,C].
-    impl: "umma" = wgmma kernel for masked windows (default), "mma" = warp-level mma.sync baseline."""
+    impl: "umma" = wgmma kernel for masked windows (default), "mma" = warp-level mma.sync baseline.  fp16 qkv / pool_kv (the
+    half-operand Linear outputs): fp16 out from the fp16 kernels (impl is then ignored: there is one fp16 plan)."""
+    dt = qkv.dtype
     if out is None:
-        out = torch.empty(t, NT, C, device=qkv.device, dtype=torch.float32)
+        out = torch.empty(t, NT, C, device=qkv.device, dtype=dt)
     prm = PPAttnParams()
     prm.qkv, prm.pool = qkv.data_ptr(), pool_kv.data_ptr()
     prm.key_tok, prm.flags, prm.out = key_tok.data_ptr(), flags.data_ptr(), out.data_ptr()
@@ -405,20 +408,29 @@ def sparse_window_attn(qkv, pool_kv, key_tok, flags, t, NT, kf_start, kf_step, o
     if prm.nkf == 0:
         out.zero_()                 # empty key set: masked windows yield zeros (softmax over an empty dim), see the C entry
     prm.scale_log2 = LOG2E / math.sqrt(128.0)
-    for tns, dt in ((qkv, torch.float32), (pool_kv, torch.float32), (key_tok, torch.int32), (flags, torch.int32)):
-        _p(_dense(tns), dt)
-    fn = _lib.lib().pp_sparse_window_attn if impl == "umma" else _lib.lib().pp_sparse_window_attn_mma
-    check(fn(ctypes.byref(prm), key_tok.shape[0], _stream()), "pp_sparse_window_attn")
+    for tns, tdt in ((qkv, dt), (pool_kv, dt), (out, dt), (key_tok, torch.int32), (flags, torch.int32)):
+        _p(_dense(tns) if tns is not out else tns, tdt)
+    if dt == torch.float16:
+        fn, name = _lib.lib().pp_sparse_window_attn_f16, "pp_sparse_window_attn_f16"
+    else:
+        fn, name = (_lib.lib().pp_sparse_window_attn if impl == "umma" else _lib.lib().pp_sparse_window_attn_mma), "pp_sparse_window_attn"
+    check(fn(ctypes.byref(prm), key_tok.shape[0], _stream()), name)
     _count(2)
     return out
 
 
 def ffn_overlap_add(Y, frames, h, w, CH=40):
-    """Y [frames*fh*fw, 49*CH] (tap-major columns) -> gelu(unfold(fold(Y)/norm)) same shape."""
+    """Y [frames*fh*fw, 49*CH] (tap-major columns) -> gelu(unfold(fold(Y)/norm)) same shape and dtype.  fp16 Y (the
+    half-operand fc1 output): fp16 Z, summed in fp32 and rounded once."""
     L = _lib.lib()
     Z = torch.empty_like(Y)
     ws_bytes = L.pp_ffn_overlap_add_workspace_bytes(frames, h, w, CH)
     ws = torch.empty(ws_bytes // 4, device=Y.device, dtype=torch.float32)
+    if Y.dtype == torch.float16:
+        check(L.pp_ffn_overlap_add_f16(_p(_dense(Y), torch.float16), Y.shape[-1], _p(Z, torch.float16), Z.shape[-1], frames, h, w, CH,
+                                       _p(ws), ws_bytes, _stream()), "pp_ffn_overlap_add_f16")
+        _count(2)
+        return Z
     check(L.pp_ffn_overlap_add(_p(_dense(Y)), Y.shape[-1], _p(Z), Z.shape[-1], frames, h, w, CH, _p(ws), ws_bytes,
                                _stream()), "pp_ffn_overlap_add")
     _count(2)
@@ -540,21 +552,32 @@ def bias_act_(x_pm, bias, act="none", slope=0.0):
 
 
 def pool_depthwise(x_pm, w_taps, bias, kh, kw):
-    """depthwise conv, kernel = stride = (kh,kw): x_pm [n,H,W,C] -> [n,H//kh,W//kw,C]; w_taps [kh*kw, C]."""
+    """depthwise conv, kernel = stride = (kh,kw): x_pm [n,H,W,C] -> [n,H//kh,W//kw,C]; w_taps [kh*kw, C].  fp16 x_pm (the
+    half-operand LayerNorm output): fp16 out, weights / bias / sums fp32."""
     n, H, W, C = x_pm.shape
-    xp, ld = _pm(x_pm)
-    out = torch.empty(n, (H - kh) // kh + 1, (W - kw) // kw + 1, C, device=x_pm.device, dtype=torch.float32)
-    check(_lib.lib().pp_pool_depthwise(xp, ld, _p(_dense(w_taps)), _p(bias), _p(out), n, H, W, C, kh, kw, _stream()),
-          "pp_pool_depthwise")
+    xp, ld = _pm(x_pm, x_pm.dtype)
+    out = torch.empty(n, (H - kh) // kh + 1, (W - kw) // kw + 1, C, device=x_pm.device, dtype=x_pm.dtype)
+    fn, name = ((_lib.lib().pp_pool_depthwise_f16, "pp_pool_depthwise_f16") if x_pm.dtype == torch.float16 else
+                (_lib.lib().pp_pool_depthwise, "pp_pool_depthwise"))
+    check(fn(xp, ld, _p(_dense(w_taps)), _p(bias), _p(out, x_pm.dtype), n, H, W, C, kh, kw, _stream()), name)
     _count(1)
     return out
 
 
-def add_layernorm(x, delta, gamma, beta, eps=1e-5):
-    """(x + delta, LayerNorm(x + delta)) over the last dim; delta=None -> (x, LayerNorm(x)).  Dense tensors."""
+def add_layernorm(x, delta, gamma, beta, eps=1e-5, y_dtype=torch.float32):
+    """(x + delta, LayerNorm(x + delta)) over the last dim; delta=None -> (x, LayerNorm(x)).  Dense tensors.  x fp32; delta
+    fp32 or fp16 (the half-operand fc2 output); y in y_dtype, fp32 or fp16 (the half-operand fc1 operand)."""
     C = x.shape[-1]
-    y = torch.empty_like(x)
+    y = torch.empty_like(x, dtype=y_dtype)
     xo = torch.empty_like(x) if delta is not None else None
+    if torch.float16 in (y_dtype, delta.dtype if delta is not None else None):
+        dt = delta.dtype if delta is not None else torch.float32
+        check(_lib.lib().pp_add_layernorm_f16(_p(_dense(x)), _p(_dense(delta), dt) if delta is not None else None,
+                                              int(dt == torch.float16), _p(gamma), _p(beta), _p(xo), _p(y, y_dtype),
+                                              int(y_dtype == torch.float16), x.numel() // C, C, float(eps), _stream()),
+              "pp_add_layernorm_f16")
+        _count(1)
+        return (xo if delta is not None else x), y
     check(_lib.lib().pp_add_layernorm(_p(_dense(x)), _p(_dense(delta)) if delta is not None else None, _p(gamma), _p(beta),
                                       _p(xo), _p(y), x.numel() // C, C, float(eps), _stream()), "pp_add_layernorm")
     _count(1)
