@@ -81,6 +81,16 @@ size_t pp_img_prop_scan_workspace_bytes(int t, int H, int W);
 int pp_img_prop_scan(const float* frames, const float* flows_f, const float* flows_b, const float* masks,
                      float* out_frames, float* out_masks, void* workspace, size_t ws_bytes, int t, int H, int W,
                      int nearest, cudaStream_t stream);
+/* The same scan on half-precision clip storage (InferenceConfig.half_storage), with the compositing of
+ * inference_propainter.py:372, 389-390, 402 in its epilogue.  frames_u8 uint8 [t][H][W][3] (the clip's frames, masked
+ * in-kernel: u8 -> [-1,1], times 1 - masks), masks float {0,1} [t][1][H][W], flows fp16 [t-1][2][H][W].  Writes frames
+ * [lo, hi) only: out_frames fp16 [hi-lo][3][H][W] = rn16(frames * (1 - masks) + prop * masks), out_masks fp16
+ * [hi-lo][1][H][W] (exact: {0,1}).  All arithmetic fp32, one fp16 rounding per output.  fp16 pointers 2-byte aligned,
+ * masks / workspace 4-byte (PP_ERR_ALIGN); lo == hi: PP_OK without a launch. */
+size_t pp_img_prop_scan_u8h_workspace_bytes(int t, int H, int W);
+int pp_img_prop_scan_u8h(const uint8_t* frames_u8, const float* masks, const void* flows_f, const void* flows_b,
+                         void* out_frames, void* out_masks, void* workspace, size_t ws_bytes, int t, int H, int W, int lo,
+                         int hi, int nearest, cudaStream_t stream);
 /* One step's prologue of BidirectionalPropagation(learnable=True) model/propainter.py:144-166:
  * fb-check + bilinear flow_warp + the two torch.cat's.  Pixel-major features (C channels), flows /
  * masks pixel-interleaved [h][w][2].  cond = [cur | warped | fx fy | valid | m0 m1 | 0..],
@@ -146,6 +156,9 @@ int pp_flow_warp_fbcheck(const float* feat, int ld_f, const float* fprop, const 
  * [lt-1][2][H][W] -> [lt-1][H/4][W/4][2] (/4); masks planar [>=lt][1][H][W] -> pmask [lt][H/4][W/4][2]. */
 int pp_gen_prep(const float* flows_f, const float* flows_b, const float* masks_in, const float* masks_upd, float* dsf,
                 float* dsb, float* pmask, int lt, int H, int W, cudaStream_t stream);
+/* pp_gen_prep on fp16 clip-storage flows (2-byte aligned, widened on load); H = 0 or W = 0: PP_OK without a launch. */
+int pp_gen_prep_f16(const void* flows_f, const void* flows_b, const float* masks_in, const float* masks_upd, float* dsf,
+                    float* dsb, float* pmask, int lt, int H, int W, cudaStream_t stream);
 /* max_pool (model/propainter.py:349-350) + window max-pool/sum (sparse_transformer.py:224-229):
  * flags[nwh*nww] = 1 if any local frame has mask inside the window. */
 int pp_window_mask(const float* pmask, int lt, int h, int w, int fh, int fw, int nwh, int nww, int* flags,

@@ -64,6 +64,9 @@ SIGNATURES = {
     "pp_img_prop_scan_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "pp_img_prop_scan": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_int,
                                  c_int, c_int, c_int, c_void_p]),
+    "pp_img_prop_scan_u8h_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "pp_img_prop_scan_u8h": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int,
+                                     c_int, c_int, c_int, c_int, c_void_p]),
     "pp_prop_cond": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                              c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "pp_deform_align_workspace_bytes": (c_size_t, [c_int, c_int]),
@@ -77,6 +80,8 @@ SIGNATURES = {
                                      c_int, c_void_p]),
     "pp_gen_prep": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                             c_void_p]),
+    "pp_gen_prep_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                c_void_p]),
     "pp_window_mask": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "pp_sparse_window_attn": (c_int, [ctypes.POINTER(PPAttnParams), c_int, c_void_p]),
     "pp_sparse_window_attn_mma": (c_int, [ctypes.POINTER(PPAttnParams), c_int, c_void_p]),

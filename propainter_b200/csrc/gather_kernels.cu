@@ -52,6 +52,89 @@ extern "C" int pp_img_prop_scan(const float* frames, const float* flows_f, const
   return PP_OK;
 }
 
+// ---- the same scan on half-precision clip storage (InferenceConfig.half_storage)
+// One step, one pixel.  The current frame is the masked uint8 frame, frames * (1 - masks) widened here (cur == nullptr: a
+// backward step), or the backward scan's fp32 result (cur: a forward step).  prev == nullptr: the first frame of a
+// direction, copied through (:141-143).  out16 != nullptr: the frame is in the kept range, and the step's epilogue stores
+// the composited frame and the updated mask, each rounded once to fp16.  The recurrent state (out, mout) stays fp32.
+__global__ void __launch_bounds__(256) k_imgprop_step_u8h(int H, int W, const uint8_t* __restrict__ u8,
+    const float* __restrict__ md, const float* __restrict__ cur, const float* __restrict__ mcur,
+    const float* __restrict__ prev, const float* __restrict__ mprev, const __half* __restrict__ fprop,
+    const __half* __restrict__ fcheck, float* __restrict__ out, float* __restrict__ mout, __half* __restrict__ out16,
+    __half* __restrict__ mout16, int nearest) {
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  const int HW = H * W;
+  if (pix >= HW) return;
+  const float m = md[pix];
+  float fr[3], cv[3], ov[3];
+  for (int c = 0; c < 3; ++c) {
+    fr[c] = pp_u8_frame(u8[3 * (long)pix + c]);
+    cv[c] = cur ? cur[(long)c * HW + pix] : PP_MUL(fr[c], PP_SUB(1.0f, m));   // frames * (1 - masks_dilated)
+  }
+  float mo = mcur ? mcur[pix] : m;
+  if (prev) mo = pp_imgprop_values(pix, H, W, cv, mo, prev, mprev, fprop, fcheck, ov, nearest);
+  else for (int c = 0; c < 3; ++c) ov[c] = cv[c];
+  if (out) {
+    for (int c = 0; c < 3; ++c) out[(long)c * HW + pix] = ov[c];
+    mout[pix] = mo;
+  }
+  if (out16) {
+    for (int c = 0; c < 3; ++c) out16[(long)c * HW + pix] = __float2half_rn(pp_imgprop_compose(fr[c], ov[c], m));
+    mout16[pix] = __float2half_rn(mo);
+  }
+}
+
+extern "C" size_t pp_img_prop_scan_u8h_workspace_bytes(int t, int H, int W) {
+  return ((size_t)t + 2) * 4 * H * W * sizeof(float);
+}
+
+// pp_img_prop_scan on clip storage, composited (model/propainter.py:315-317; inference_propainter.py:372, 389-390, 402):
+// see include/propainter_b200.h
+extern "C" int pp_img_prop_scan_u8h(const uint8_t* frames_u8, const float* masks, const void* flows_f, const void* flows_b,
+                                    void* out_frames, void* out_masks, void* workspace, size_t ws_bytes, int t, int H, int W,
+                                    int lo, int hi, int nearest, cudaStream_t stream) {
+  if (t < 0 || H < 2 || W < 2 || lo < 0 || lo > hi || hi > t) return PP_ERR_SHAPE;
+  if (((uintptr_t)flows_f | (uintptr_t)flows_b | (uintptr_t)out_frames | (uintptr_t)out_masks) & 1) return PP_ERR_ALIGN;
+  if (((uintptr_t)masks | (uintptr_t)workspace) & 3) return PP_ERR_ALIGN;
+  if (lo == hi) return PP_OK;                                // nothing kept: no launch
+  if (ws_bytes < pp_img_prop_scan_u8h_workspace_bytes(t, H, W)) return PP_ERR_WORKSPACE;
+  const long HW = (long)H * W;
+  const __half* ff = (const __half*)flows_f;
+  const __half* fb = (const __half*)flows_b;
+  __half* of = (__half*)out_frames;
+  __half* om = (__half*)out_masks;
+  float* bf = (float*)workspace;             // backward-scan frames [t][3][HW]
+  float* bm = bf + (long)t * 3 * HW;         // backward-scan masks  [t][HW]
+  float* rf = bm + (long)t * HW;             // forward-scan state, a two-frame ring: frames [2][3][HW]
+  float* rm = rf + 2 * 3 * HW;               //                                       masks  [2][HW]
+  const int blocks = pp_blocks(HW, 256);
+#define PP_U8(i) (frames_u8 + (long)(i) * 3 * HW)
+#define PP_MD(i) (masks + (long)(i) * HW)
+  // backward scan: t-1 -> 0, propagates along the forward flows
+  k_imgprop_step_u8h<<<blocks, 256, 0, stream>>>(H, W, PP_U8(t - 1), PP_MD(t - 1), nullptr, nullptr, nullptr, nullptr,
+      nullptr, nullptr, bf + (long)(t - 1) * 3 * HW, bm + (long)(t - 1) * HW, nullptr, nullptr, nearest);
+  for (int i = t - 2; i >= 0; --i)
+    k_imgprop_step_u8h<<<blocks, 256, 0, stream>>>(H, W, PP_U8(i), PP_MD(i), nullptr, nullptr,
+        bf + (long)(i + 1) * 3 * HW, bm + (long)(i + 1) * HW, ff + (long)i * 2 * HW, fb + (long)i * 2 * HW,
+        bf + (long)i * 3 * HW, bm + (long)i * HW, nullptr, nullptr, nearest);
+  // forward scan: consumes the backward scan's frames and masks (:138-139); frame 0 is the backward result itself
+  if (lo == 0)
+    k_imgprop_step_u8h<<<blocks, 256, 0, stream>>>(H, W, PP_U8(0), PP_MD(0), bf, bm, nullptr, nullptr, nullptr, nullptr,
+        nullptr, nullptr, of, om, nearest);
+  for (int i = 1; i < hi; ++i) {
+    const float* pf = i == 1 ? bf : rf + (long)((i - 1) & 1) * 3 * HW;
+    const float* pm = i == 1 ? bm : rm + (long)((i - 1) & 1) * HW;
+    const bool keep = i >= lo;
+    k_imgprop_step_u8h<<<blocks, 256, 0, stream>>>(H, W, PP_U8(i), PP_MD(i), bf + (long)i * 3 * HW, bm + (long)i * HW,
+        pf, pm, fb + (long)(i - 1) * 2 * HW, ff + (long)(i - 1) * 2 * HW, rf + (long)(i & 1) * 3 * HW, rm + (long)(i & 1) * HW,
+        keep ? of + (long)(i - lo) * 3 * HW : nullptr, keep ? om + (long)(i - lo) * HW : nullptr, nearest);
+  }
+#undef PP_U8
+#undef PP_MD
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+
 // ================================================================ learnable propagation: cond assembly
 // One warp per pixel: lane 0 evaluates the sampling coordinate + fb-consistency and broadcasts it by
 // shuffle; the 32 lanes then gather the 4 bilinear corners as float4 channel vectors (coalesced 512 B
@@ -280,7 +363,8 @@ extern "C" int pp_convex_upsample(const float* mask, int ld_mask, float mask_sca
 }
 
 // ================================================================ generator input preparation
-__global__ void __launch_bounds__(256) k_gen_prep(const float* __restrict__ flows_f, const float* __restrict__ flows_b,
+template <typename TF>
+__global__ void __launch_bounds__(256) k_gen_prep(const TF* __restrict__ flows_f, const TF* __restrict__ flows_b,
     const float* __restrict__ masks_in, const float* __restrict__ masks_upd, float* __restrict__ dsf,
     float* __restrict__ dsb, float* __restrict__ pmask, int lt, int H, int W) {
   const int h = H / 4, w = W / 4;
@@ -290,7 +374,7 @@ __global__ void __launch_bounds__(256) k_gen_prep(const float* __restrict__ flow
   int f = (int)(i / per); int r = (int)(i - (long)f * per); int y = r / w, x = r - y * w;
   const long HW = (long)H * W;
   if (f < lt - 1) {
-    const float* pf = flows_f + (long)f * 2 * HW; const float* pb = flows_b + (long)f * 2 * HW;
+    const TF* pf = flows_f + (long)f * 2 * HW; const TF* pb = flows_b + (long)f * 2 * HW;
     dsf[2 * i] = pp_flow_ds4(pf, W, y, x); dsf[2 * i + 1] = pp_flow_ds4(pf + HW, W, y, x);
     dsb[2 * i] = pp_flow_ds4(pb, W, y, x); dsb[2 * i + 1] = pp_flow_ds4(pb + HW, W, y, x);
   }
@@ -303,7 +387,20 @@ extern "C" int pp_gen_prep(const float* flows_f, const float* flows_b, const flo
                            float* dsf, float* dsb, float* pmask, int lt, int H, int W, cudaStream_t stream) {
   if (H % 4 || W % 4 || lt < 1) return PP_ERR_SHAPE;
   long n = (long)lt * (H / 4) * (W / 4);
-  k_gen_prep<<<pp_blocks(n, 256), 256, 0, stream>>>(flows_f, flows_b, masks_in, masks_upd, dsf, dsb, pmask, lt, H, W);
+  k_gen_prep<float><<<pp_blocks(n, 256), 256, 0, stream>>>(flows_f, flows_b, masks_in, masks_upd, dsf, dsb, pmask, lt, H, W);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+// the same on fp16 clip-storage flows (2-byte aligned), widened on load
+extern "C" int pp_gen_prep_f16(const void* flows_f, const void* flows_b, const float* masks_in, const float* masks_upd,
+                               float* dsf, float* dsb, float* pmask, int lt, int H, int W, cudaStream_t stream) {
+  if (H < 0 || W < 0 || H % 4 || W % 4 || lt < 1) return PP_ERR_SHAPE;
+  if (((uintptr_t)flows_f | (uintptr_t)flows_b) & 1) return PP_ERR_ALIGN;
+  if (((uintptr_t)masks_in | (uintptr_t)masks_upd | (uintptr_t)dsf | (uintptr_t)dsb | (uintptr_t)pmask) & 3) return PP_ERR_ALIGN;
+  const long n = (long)lt * (H / 4) * (W / 4);
+  if (n == 0) return PP_OK;                                  // an empty frame: no launch
+  k_gen_prep<__half><<<pp_blocks(n, 256), 256, 0, stream>>>((const __half*)flows_f, (const __half*)flows_b, masks_in, masks_upd,
+                                                            dsf, dsb, pmask, lt, H, W);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }
@@ -990,8 +1087,7 @@ __global__ void __launch_bounds__(256) k_u8_to_frames(const uint8_t* __restrict_
   long HW = (long)H * W;
   if (i >= (long)T * 3 * HW) return;
   long f = i / (3 * HW); long r = i - f * 3 * HW; int c = (int)(r / HW); long p = r - (long)c * HW;
-  float v = PP_DIV((float)src[(f * HW + p) * 3 + c], 255.0f);
-  dst[i] = PP_SUB(PP_MUL(v, 2.0f), 1.0f);
+  dst[i] = pp_u8_frame(src[(f * HW + p) * 3 + c]);
 }
 // replaces to_tensors()(frames)*2-1 (core/utils.py:130-170, inference_propainter.py:264)
 extern "C" int pp_u8_to_frames(const uint8_t* src, float* dst, int T, int H, int W, cudaStream_t stream) {

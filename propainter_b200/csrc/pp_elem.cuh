@@ -4,6 +4,32 @@
 #include "pp_common.cuh"
 
 // ------------------------------------------------------------------------------------------------
+// Half-precision clip storage (InferenceConfig.half_storage): fp16 tensors between stages, widened exactly to fp32 on
+// load, so every rule below computes in fp32 whatever the storage dtype.  The host build has no cuda_fp16.h: there an
+// fp16 value is its IEEE binary16 bit pattern.
+#if defined(PP_HOSTSIM)
+struct pp_half { uint16_t bits; };
+PP_HD float pp_widen(pp_half h) {
+  const uint32_t s = (uint32_t)(h.bits & 0x8000u) << 16, e = (h.bits >> 10) & 0x1fu, m = h.bits & 0x3ffu;
+  if (e == 0) {                                                   // zero / subnormal: m * 2^-24, exact in fp32
+    const float v = ldexpf((float)m, -24);
+    return s ? -v : v;
+  }
+  union { uint32_t u; float f; } r;
+  r.u = s | (e == 31 ? 0x7f800000u : (e + 112u) << 23) | (m << 13);
+  return r.f;
+}
+#else
+typedef __half pp_half;
+PP_HD float pp_widen(__half h) { return __half2float(h); }
+#endif
+PP_HD float pp_widen(float v) { return v; }
+
+// to_tensors()(frames) * 2 - 1 of one uint8 channel value (core/utils.py:130-170, inference_propainter.py:264): the
+// frame conversion of pp_u8_to_frames and the in-kernel widening of pp_img_prop_scan_u8h
+PP_HD float pp_u8_frame(uint8_t v) { return PP_SUB(PP_MUL(PP_DIV((float)v, 255.0f), 2.0f), 1.0f); }
+
+// ------------------------------------------------------------------------------------------------
 // grid_sample coordinate round trip.
 // flow_warp (model/modules/flow_loss_utils.py:34-37): g = 2*(p+f)/max(size-1,1) - 1, then ATen's
 // align_corners=True un-normalisation ((g+1)/2)*(size-1).  Kept as separate roundings so that
@@ -41,16 +67,18 @@ PP_HD PPTaps pp_taps(float ix, float iy, int H, int W) {
   t.w11 = (yh && xh) ? wx1 * wy1 : 0.f;
   return t;
 }
-// sample one scalar plane [H][ld] through a tap set (order nw, ne, sw, se like ATen)
-PP_HD float pp_tap_plane(const float* p, int ld, const PPTaps& t) {
+// sample one scalar plane [H][ld] (fp32, or fp16 clip storage widened on load) through a tap set (order nw, ne, sw, se
+// like ATen)
+template <typename T>
+PP_HD float pp_tap_plane(const T* p, int ld, const PPTaps& t) {
   if (!t.any) return 0.f;
   float acc = 0.f;
-  const float* r0 = p + (long)t.y0 * ld + t.x0;
-  const float* r1 = r0 + ld;
-  if (t.w00 != 0.f) acc += r0[0] * t.w00;
-  if (t.w01 != 0.f) acc += r0[1] * t.w01;
-  if (t.w10 != 0.f) acc += r1[0] * t.w10;
-  if (t.w11 != 0.f) acc += r1[1] * t.w11;
+  const T* r0 = p + (long)t.y0 * ld + t.x0;
+  const T* r1 = r0 + ld;
+  if (t.w00 != 0.f) acc += pp_widen(r0[0]) * t.w00;
+  if (t.w01 != 0.f) acc += pp_widen(r0[1]) * t.w01;
+  if (t.w10 != 0.f) acc += pp_widen(r1[0]) * t.w10;
+  if (t.w11 != 0.f) acc += pp_widen(r1[1]) * t.w11;
   return acc;
 }
 // nearest (round-half-to-even, zeros padding): returns linear index or -1
@@ -71,20 +99,20 @@ PP_HD float pp_fb_valid(float fx, float fy, float bx, float by) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// One step of the non-learnable image propagation scan (model/propainter.py:144-161), one pixel.
-// All tensors planar: frames 3 planes of H*W, masks/flows likewise.  `nearest` selects :149's mode.
-PP_HD void pp_imgprop_pixel(int pix, int H, int W, const float* cur, const float* mcur, const float* prev,
-                            const float* mprev, const float* fprop, const float* fcheck, float* out,
-                            float* mout, int nearest) {
+// One step of the non-learnable image propagation scan (model/propainter.py:144-161), one pixel, in value form: cv the
+// pixel's current frame (3 channels), mc its current mask; writes the step's frame values to ov and returns its mask.
+// prev / mprev / flows planar ([3][H*W], [H*W], [2][H*W]); flows fp32 or fp16.  `nearest` selects :149's mode.
+template <typename TF>
+PP_HD float pp_imgprop_values(int pix, int H, int W, const float* cv, float mc, const float* prev, const float* mprev,
+                              const TF* fprop, const TF* fcheck, float* ov, int nearest) {
   const int HW = H * W;
   int y = pix / W, x = pix - y * W;
-  float fx = fprop[pix], fy = fprop[HW + pix];
+  float fx = pp_widen(fprop[pix]), fy = pp_widen(fprop[HW + pix]);
   float ix = pp_warp_coord((float)x, fx, W), iy = pp_warp_coord((float)y, fy, H);
   PPTaps t = pp_taps(ix, iy, H, W);
   float bx = pp_tap_plane(fcheck, W, t), by = pp_tap_plane(fcheck + HW, W, t);
   float valid = pp_fb_valid(fx, fy, bx, by);
   float mw = pp_tap_plane(mprev, W, t) > 0.1f ? 1.0f : 0.0f;            // binary_mask(:156)
-  float mc = mcur[pix];
   float gate = PP_MUL(PP_MUL(mc, valid), PP_SUB(1.0f, mw));
   float use = gate > 0.1f ? 1.0f : 0.0f;                                 // :158
   long ni = nearest ? pp_nearest_index(ix, iy, H, W, W) : 0;
@@ -92,11 +120,26 @@ PP_HD void pp_imgprop_pixel(int pix, int H, int W, const float* cur, const float
     float wv;
     if (nearest) wv = ni >= 0 ? prev[(long)c * HW + ni] : 0.f;
     else wv = pp_tap_plane(prev + (long)c * HW, W, t);
-    float cv = cur[(long)c * HW + pix];
-    out[(long)c * HW + pix] = PP_ADD(PP_MUL(use, wv), PP_MUL(PP_SUB(1.0f, use), cv));   // :159
+    ov[c] = PP_ADD(PP_MUL(use, wv), PP_MUL(PP_SUB(1.0f, use), cv[c]));   // :159
   }
   float m2 = PP_MUL(mc, PP_SUB(1.0f, PP_MUL(valid, PP_SUB(1.0f, mw))));  // :161
-  mout[pix] = m2 > 0.1f ? 1.0f : 0.0f;
+  return m2 > 0.1f ? 1.0f : 0.0f;
+}
+// the same step on planar fp32 frames: cur, out [3][H*W]; mcur, mout [H*W]
+PP_HD void pp_imgprop_pixel(int pix, int H, int W, const float* cur, const float* mcur, const float* prev,
+                            const float* mprev, const float* fprop, const float* fcheck, float* out,
+                            float* mout, int nearest) {
+  const int HW = H * W;
+  const float cv[3] = {cur[pix], cur[HW + pix], cur[2 * HW + pix]};
+  float ov[3];
+  const float m = pp_imgprop_values(pix, H, W, cv, mcur[pix], prev, mprev, fprop, fcheck, ov, nearest);
+  for (int c = 0; c < 3; ++c) out[(long)c * HW + pix] = ov[c];
+  mout[pix] = m;
+}
+// The updated frame of one channel (inference_propainter.py:389-390, :402; ProPainterPipeline.propagate_images):
+// frames * (1 - masks) + prop * masks in the torch expression's order, one rounding per operation.
+PP_HD float pp_imgprop_compose(float frame, float prop, float m) {
+  return PP_ADD(PP_MUL(frame, PP_SUB(1.0f, m)), PP_MUL(prop, m));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -285,10 +328,12 @@ PP_HD float2 pp_convex_up(const float* mask_px, float mask_scale, const float* f
 // ------------------------------------------------------------------------------------------------
 // InpaintGenerator.forward down-sampling (propainter.py:338-342; stencils pinned in SURVEY.md §8c):
 // bilinear 1/4 (align_corners=False) == mean of the centre 2x2 of each 4x4 block; then /4.
-PP_HD float pp_flow_ds4(const float* plane, int W, int y, int x) {
-  const float* p = plane + (long)(4 * y + 1) * W + 4 * x + 1;
-  float top = 0.5f * p[0] + 0.5f * p[1];
-  float bot = 0.5f * p[W] + 0.5f * p[W + 1];
+// The flow plane is fp32 or fp16 clip storage (widened on load).
+template <typename T>
+PP_HD float pp_flow_ds4(const T* plane, int W, int y, int x) {
+  const T* p = plane + (long)(4 * y + 1) * W + 4 * x + 1;
+  float top = 0.5f * pp_widen(p[0]) + 0.5f * pp_widen(p[1]);
+  float bot = 0.5f * pp_widen(p[W]) + 0.5f * pp_widen(p[W + 1]);
   return PP_DIV(0.5f * top + 0.5f * bot, 4.0f);
 }
 

@@ -179,6 +179,8 @@ class ShardedProPainter:
         """Returns (comp_u8 [n,H,W,3], frame_ids): the composited frames whose final value this rank holds (ascending).
         gather=True additionally assembles the whole video on every rank (tests; costs a collective over the output)."""
         cfg = cfg or InferenceConfig()
+        if getattr(cfg, "half_storage", False):
+            raise ValueError("the sharded runner keeps fp32 clip storage: InferenceConfig.half_storage is not supported here")
         pipe, dev, rank = self.pipe, self.pipe.device, self.rank
         self.last_bytes = {}
         ori = frames_u8.to(dev, non_blocking=True)

@@ -148,12 +148,17 @@ def evaluate_flow_clip(pipe, frames_u8, masks_u8, reference_flows=None, cfg=None
     fr = torch.as_tensor(frames_u8).to(dev)
     mk = torch.as_tensor(masks_u8).to(dev)
     fm, _ = prepare_masks(((mk != 0).to(torch.uint8) * 255).contiguous(), mask_dilation, dev)
-    gt =pipe.compute_flows(ops.u8_to_frames(fr).unsqueeze(0), cfg)
+    if cfg.half_storage:                       # fp16 RAFT flows in, fp16 completed flows out (InferenceConfig.half_storage)
+        gt = pipe.compute_flows_half(fr.contiguous(), cfg)
+    else:
+        gt =pipe.compute_flows(ops.u8_to_frames(fr).unsqueeze(0), cfg)
     net = pipe.fix_flow_complete
     torch.cuda.synchronize(dev)
     t0 = time.perf_counter()
     pred, _ = net.forward_bidirect_flow(gt, fm)
     pred = net.combine_flow(gt, pred, fm)
+    if cfg.half_storage:
+        pred = tuple(p.half() for p in pred)
     torch.cuda.synchronize(dev)
     dt = time.perf_counter() - t0
     ref = gt if reference_flows is None else tuple(torch.as_tensor(r).to(dev).float().reshape(p.shape)

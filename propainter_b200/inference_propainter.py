@@ -34,6 +34,11 @@ class InferenceConfig:
     # kernels here compute in fp32 whatever the storage dtype (a `.half()` net is widened once, fp16 inputs are widened at
     # entry and results handed back in the caller's dtype), so the flag is accepted and changes nothing in the pipeline.
     fp16: bool = False
+    # Half-precision clip storage: the four clip-resident stage outputs (RAFT flows, completed flows, updated frames and
+    # masks, encoder features) are rounded once to fp16 where a stage hands them on, and widened to fp32 on load; all
+    # arithmetic stays fp32.  A clip then holds about 35 instead of 95 bytes per pixel and frame (DESIGN.md §7), for a small
+    # change of the result, so it is the caller's explicit choice (the reference's --fp16 "to reduce running memory cost").
+    half_storage: bool = False
 
 
 def get_ref_index(mid_neighbor_id, neighbor_ids, length, ref_stride=10, ref_num=-1):
@@ -206,6 +211,51 @@ class ProPainterPipeline:
             umk.append(um[:, lo:hi])
         return torch.cat(uf, 1), torch.cat(umk, 1)
 
+    # ---- stages 1-3 on half-precision clip storage (InferenceConfig.half_storage): each stage's clip-sized output is
+    # rounded once to fp16 (R1: RAFT flows, R2: completed flows, R3: updated frames / masks) into a preallocated clip
+    # buffer, chunk by chunk; every consumer widens it to fp32
+    def compute_flows_half(self, ori_u8, cfg):
+        """stage 1 on uint8 frames [T,H,W,3]: RAFT on fp32 frames built per chunk -> fp16 (forward, backward) [1,T-1,2,H,W]"""
+        T, H, W = ori_u8.shape[0], ori_u8.shape[1], ori_u8.shape[2]
+        clip = cfg.raft_clip_frames
+        if clip is None:
+            clip = auto_clip_frames(T, H, W, self.fix_raft.fix_raft.corr_plan(H, W, ori_u8.device))
+        gf = torch.empty(1, max(T - 1, 0), 2, H, W, device=ori_u8.device, dtype=torch.float16)
+        gb = torch.empty_like(gf)
+        for s, e in flow_chunks(T, clip):
+            f, b = self.fix_raft(ops.u8_to_frames(ori_u8[s:e]).unsqueeze(0), iters=cfg.raft_iter)
+            gf[:, s:e - 1].copy_(f)
+            gb[:, s:e - 1].copy_(b)
+        return gf, gb
+
+    def complete_flows_half(self, gt_flows, flow_masks, cfg):
+        """stage 2 on fp16 RAFT flows: each sub-video is widened inside the net, and its kept range of the combined flows is
+        rounded into fp16 clip buffers"""
+        net, L = self.fix_flow_complete, gt_flows[0].shape[1]
+        out = (torch.empty_like(gt_flows[0]), torch.empty_like(gt_flows[1]))
+        units = [(0, L, 0, L)] if L <= cfg.subvideo_length else halo_chunks(L, cfg.subvideo_length, 5)
+        for s, e, lo, hi in units:
+            sub = (gt_flows[0][:, s:e], gt_flows[1][:, s:e])
+            pred, _ = net.forward_bidirect_flow(sub, flow_masks[:, s:e + 1])
+            pred = net.combine_flow(sub, pred, flow_masks[:, s:e + 1])
+            out[0][:, s + lo:s + hi].copy_(pred[0][:, lo:hi])
+            out[1][:, s + lo:s + hi].copy_(pred[1][:, lo:hi])
+        return out
+
+    def propagate_images_half(self, ori_u8, masks_dilated, pred_flows, cfg):
+        """stage 3 on the clip's uint8 frames and fp16 completed flows: one pp_img_prop_scan_u8h call per sub-video masks the
+        frames, runs the fp32 scan and writes its kept frames, composited, into fp16 clip buffers [1,T,3,H,W] / [1,T,1,H,W]"""
+        T, H, W = ori_u8.shape[0], ori_u8.shape[1], ori_u8.shape[2]
+        md = masks_dilated[0].contiguous()
+        uf = torch.empty(1, T, 3, H, W, device=ori_u8.device, dtype=torch.float16)
+        um = torch.empty(1, T, 1, H, W, device=ori_u8.device, dtype=torch.float16)
+        sub = min(100, cfg.subvideo_length)
+        units = [(0, T, 0, T)] if T <= sub else halo_chunks(T, sub, 10)
+        for s, e, lo, hi in units:
+            ops.img_prop_scan_u8h(ori_u8[s:e], md[s:e], pred_flows[0][0, s:e - 1], pred_flows[1][0, s:e - 1],
+                                  uf[0, s + lo:s + hi], um[0, s + lo:s + hi], lo, hi)
+        return uf, um
+
     # ---- stage 4 (:406-452)
     def generate(self, upd_frames, masks_dilated, upd_masks, pred_flows, ori_u8, cfg, windows=None, comp=None,
                  visited=None):
@@ -215,7 +265,12 @@ class ProPainterPipeline:
         visited = [False] * T if visited is None else visited
         md = masks_dilated[0].contiguous()
         # encoder features depend only on (frame, mask, updated mask): computed once per clip, not once per window
-        enc_all = self.model.encode(upd_frames[0], md, upd_masks[0]).permute(0, 2, 3, 1)     # pixel-major rows: cheap frame gather
+        if cfg.half_storage:                                       # R4: fp16 pixel-major clip buffer, widened per window
+            H, W = upd_frames.shape[-2:]
+            enc_all = self.model.encode(upd_frames[0], md, upd_masks[0], out=torch.empty(
+                T, H // 4, W // 4, 128, device=upd_frames.device, dtype=torch.float16))
+        else:
+            enc_all = self.model.encode(upd_frames[0], md, upd_masks[0]).permute(0, 2, 3, 1)  # pixel-major rows: cheap frame gather
         todo = [(wi, nb, refs) for wi, (nb, refs) in enumerate(plan) if windows is None or wi in windows]
 
         um0 = upd_masks[0]
@@ -226,7 +281,7 @@ class ProPainterPipeline:
             # (measured: generate() blocked the host for the whole clip, so nothing could be queued behind it)
             idx = self.index(nb + refs)
             a, b = nb[0], nb[-1]                                   # neighbour frames are a contiguous range
-            return lambda slot: self.model.forward_features(enc_all.index_select(0, idx).permute(0, 3, 1, 2),
+            return lambda slot: self.model.forward_features(enc_all.index_select(0, idx).float().permute(0, 3, 1, 2),
                                                             (pred_flows[0][0, a:b], pred_flows[1][0, a:b]),
                                                             md.index_select(0, idx), um0.index_select(0, idx), len(nb), slot=slot)
 
@@ -283,6 +338,17 @@ class ProPainterPipeline:
         ori = frames_u8.to(dev, non_blocking=True)
         flow_masks = flow_masks.to(dev, non_blocking=True).float()
         masks_dilated = masks_dilated.to(dev, non_blocking=True).float()
+        if cfg.half_storage:
+            # no clip-sized fp32 frames: RAFT builds them per chunk, stage 3 masks the uint8 frames in its kernel
+            gt = self.compute_flows_half(ori, cfg)
+            pred = self.complete_flows_half(gt, flow_masks, cfg)
+            stages = {"gt_flows": gt} if return_stages else {}
+            del gt                                                 # released after stage 2 unless it is returned
+            upd_f, upd_m = self.propagate_images_half(ori, masks_dilated, pred, cfg)
+            comp = self.generate(upd_f, masks_dilated, upd_m, pred, ori, cfg)
+            if return_stages:
+                return comp, dict(stages, pred_flows=pred, updated_frames=upd_f, updated_masks=upd_m)
+            return comp
         frames = ops.u8_to_frames(ori).unsqueeze(0)
         gt = self.compute_flows(frames, cfg)
         pred = self.complete_flows(gt, flow_masks, cfg)
@@ -312,11 +378,14 @@ class ProPainterPipeline:
         """Stages 1-2 only (inference_propainter.py:302-368): RAFT flows and the completed flows, with the chunking of
         __call__ and without image propagation or the generator.  frames_u8 uint8 [T,H,W,3] (host or device), flow_masks
         float {0,1} [1,T,1,H,W].  Returns (gt_flows, pred_flows), each a (forward, backward) pair of [1,T-1,2,H,W],
-        bit-identical to the stage outputs of __call__(..., return_stages=True)."""
+        bit-identical to the stage outputs of __call__(..., return_stages=True); fp16 with cfg.half_storage."""
         cfg = cfg or InferenceConfig()
         dev = self.device
         ori = torch.as_tensor(frames_u8).to(dev, non_blocking=True)
         flow_masks = flow_masks.to(dev, non_blocking=True).float()
+        if cfg.half_storage:
+            gt = self.compute_flows_half(ori, cfg)
+            return gt, self.complete_flows_half(gt, flow_masks, cfg)
         frames = ops.u8_to_frames(ori).unsqueeze(0)
         gt = self.compute_flows(frames, cfg)
         return gt, self.complete_flows(gt, flow_masks, cfg)

@@ -34,9 +34,11 @@ class ProInpainter:
         self.pipe = ProPainterPipeline(self.fix_raft, self.fix_flow_complete, self.model, device=self.device)
 
     @torch.no_grad()
-    def inpaint(self, npframes, masks, ratio=1.0, dilate_radius=4, raft_iter=20, subvideo_length=80, neighbor_length=10, ref_stride=10):
+    def inpaint(self, npframes, masks, ratio=1.0, dilate_radius=4, raft_iter=20, subvideo_length=80, neighbor_length=10, ref_stride=10,
+                half_storage=False):
         """npframes: T x [H,W,3] uint8 (array or list); masks: T (or 1) x [H,W] (non-zero = hole).  Returns a list of T uint8
-        frames [H_out, W_out, 3] (base_inpainter.py:190-374)."""
+        frames [H_out, W_out, 3] (base_inpainter.py:190-374).  half_storage: keep the clip's stage outputs in fp16
+        (InferenceConfig.half_storage)."""
         fr = torch.from_numpy(np.ascontiguousarray(np.stack([np.asarray(f).astype(np.uint8) for f in npframes]))).to(self.device)
         T, H, W, _ = fr.shape
         out_size, size = process_sizes((W, H), ratio)
@@ -50,7 +52,7 @@ class ProInpainter:
         if dil.shape[1] == 1 and T > 1:
             dil = dil.expand(1, T, 1, size[1], size[0]).contiguous()
         cfg = InferenceConfig(raft_iter=raft_iter, ref_stride=ref_stride, neighbor_length=neighbor_length, subvideo_length=subvideo_length,
-                              fp16=self.use_half)
+                              fp16=self.use_half, half_storage=half_storage)
         comp = self.pipe(fr, dil, dil.clone(), cfg)                                  # both masks use dilate_radius (:214)
         if out_size != size:
             comp = ops.resize_output_u8(comp, out_size)                              # cv2.resize(f, out_size)

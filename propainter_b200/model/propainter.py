@@ -17,6 +17,12 @@ from ..window_index import padded_grid, token_grid
 from .modules.sparse_transformer import WIN, TransformerExec
 
 
+def _flow_in(f):
+    """a window's completed flows as gen_prep reads them: fp16 clip storage as it is (pp_gen_prep_f16 widens it on load),
+    anything else as fp32"""
+    return f.contiguous() if f.dtype == torch.float16 else f.contiguous().float()
+
+
 def _lrelu(x, s=0.2):
     return F.leaky_relu_(x, s)
 
@@ -308,16 +314,22 @@ class InpaintGenerator(ParamNet):
 
     # ------------------------------------------------------------------ forward
     @torch.no_grad()
-    def encode(self, masked_frames, masks_in, masks_updated, chunk=40):
+    def encode(self, masked_frames, masks_in, masks_updated, chunk=40, out=None):
         """Encoder features of a set of frames: [n,3,H,W], [n,1,H,W], [n,1,H,W] -> [n,128,H/4,W/4].
         The encoder output of a frame depends only on (frame, mask_in, mask_updated), so the sliding-window
         driver calls this once per clip and feeds ``forward_features``; the reference re-encodes every frame
-        in each of the ~3.5 windows that select it (propainter.py:330-333, 58 % of the generator's conv FLOPs)."""
+        in each of the ~3.5 windows that select it (propainter.py:330-333, 58 % of the generator's conv FLOPs).
+        `out` (fp16 pixel-major [n,H/4,W/4,128], half-precision clip storage): each chunk's features are rounded once
+        into it instead of being concatenated, and `out` is returned."""
         outs = []
         for s in range(0, masked_frames.shape[0], chunk):
-            outs.append(self.graphs("gen_enc", self._encode_frames, masked_frames[s:s + chunk].contiguous().float(),
-                                    masks_in[s:s + chunk].contiguous().float(), masks_updated[s:s + chunk].contiguous().float()))
-        return torch.cat(outs, 0)
+            o = self.graphs("gen_enc", self._encode_frames, masked_frames[s:s + chunk].contiguous().float(),
+                            masks_in[s:s + chunk].contiguous().float(), masks_updated[s:s + chunk].contiguous().float())
+            if out is None:
+                outs.append(o)
+            else:
+                out[s:s + o.shape[0]].copy_(o.permute(0, 2, 3, 1))
+        return torch.cat(outs, 0) if out is None else out
 
     def _encode_frames(self, fr, mi, mu):
         n, _, H, W = fr.shape
@@ -327,14 +339,14 @@ class InpaintGenerator(ParamNet):
     @torch.no_grad()
     def forward_features(self, enc_feat, completed_flows, masks_in, masks_updated, num_local_frames,
                          interpolation="bilinear", t_dilation=2, slot=0):
-        """``forward`` minus the encoder: enc_feat [t,128,h,w] (local frames first), flows 2x[lt-1,2,H,W],
+        """``forward`` minus the encoder: enc_feat [t,128,h,w] (local frames first), flows 2x[lt-1,2,H,W] (fp16 or fp32),
         masks [t,1,H,W] -> [lt,3,H,W].  `slot` selects an independent captured-graph instance so that several
         windows can be in flight on different streams."""
         lt = num_local_frames
         return self.graphs(("gen_feat", lt, interpolation, t_dilation, slot),
                            lambda *a: self._forward_features(*a, lt, interpolation, t_dilation),
-                           enc_feat.contiguous(memory_format=torch.channels_last), completed_flows[0].contiguous().float(),
-                           completed_flows[1].contiguous().float(), masks_in.contiguous().float(),
+                           enc_feat.contiguous(memory_format=torch.channels_last), _flow_in(completed_flows[0]),
+                           _flow_in(completed_flows[1]), masks_in.contiguous().float(),
                            masks_updated.contiguous().float())
 
     @torch.no_grad()

@@ -1,7 +1,8 @@
 """Tensor-level wrappers over the C ABI.  Each takes/returns torch CUDA tensors, passes raw pointers +
 the current stream, and raises on any non-zero return code.  fp32, except the fp16 operand / result tensors of RAFT's
 half-precision refinement convs (corr_lookup, bias_act, gru_gate, gru_update, raft_pack_motion) and of the transformer's
-half-operand transformer (sparse_window_attn, pool_depthwise, ffn_overlap_add, add_layernorm); DESIGN.md §4 "Precision"."""
+half-operand transformer (sparse_window_attn, pool_depthwise, ffn_overlap_add, add_layernorm); DESIGN.md §4 "Precision".  The
+half-precision clip storage (img_prop_scan_u8h, gen_prep) reads and writes fp16 tensors between stages; DESIGN.md §7."""
 import collections
 import ctypes
 import math
@@ -187,6 +188,26 @@ def img_prop_scan(frames, flows_f, flows_b, masks, nearest=True):
     return of, om
 
 
+def img_prop_scan_u8h(frames_u8, masks, flows_f, flows_b, out_frames, out_masks, lo=0, hi=None, nearest=True):
+    """img_prop_scan on half-precision clip storage, composited: frames_u8 uint8 [t,H,W,3], masks float {0,1} [t,1,H,W],
+    fp16 flows [t-1,2,H,W].  Writes frames [lo, hi) of frames * (1 - masks) + prop * masks into fp16 out_frames
+    [hi-lo,3,H,W] and of the updated masks into fp16 out_masks [hi-lo,1,H,W] (views of clip buffers); the scan is fp32."""
+    L = _lib.lib()
+    t, H, W, _ = frames_u8.shape
+    hi = t if hi is None else hi
+    if tuple(out_frames.shape) != (hi - lo, 3, H, W) or tuple(out_masks.shape) != (hi - lo, 1, H, W):
+        raise RuntimeError(f"img_prop_scan_u8h: outputs for frames [{lo}, {hi}) of a {H}x{W} clip, got "
+                           f"{tuple(out_frames.shape)} / {tuple(out_masks.shape)}")
+    ws_bytes = L.pp_img_prop_scan_u8h_workspace_bytes(t, H, W)
+    ws = torch.empty(ws_bytes // 4, device=frames_u8.device, dtype=torch.float32)
+    f16 = torch.float16
+    check(L.pp_img_prop_scan_u8h(_p(_dense(frames_u8), torch.uint8), _p(_dense(masks)), _p(_dense(flows_f), f16),
+                                 _p(_dense(flows_b), f16), _p(_dense(out_frames), f16), _p(_dense(out_masks), f16), _p(ws),
+                                 ws_bytes, t, H, W, lo, hi, int(bool(nearest)), _stream()), "pp_img_prop_scan_u8h")
+    _count(t + hi - (lo > 0) if hi > lo else 0)
+    return out_frames, out_masks
+
+
 def prop_cond(cur, prop, fprop, fcheck, mcur, cond, bb, first):
     """cur/prop [h,w,C] pixel-major views; fprop/fcheck/mcur [h,w,2]; cond [h,w,ldc]; bb [h,w,ldb]."""
     h, w, C = cur.shape
@@ -369,15 +390,19 @@ def pack_deform_weight(weight):
 
 
 def gen_prep(flows_f, flows_b, masks_in, masks_upd, lt):
-    """planar flows [lt-1,2,H,W], masks [>=lt,1,H,W] -> dsf, dsb [lt-1,h,w,2], pmask [lt,h,w,2]."""
+    """planar flows [lt-1,2,H,W] (fp32, or fp16 clip storage), masks [>=lt,1,H,W] -> dsf, dsb [lt-1,h,w,2], pmask [lt,h,w,2]."""
     H, W = masks_in.shape[-2:]
     h, w = H // 4, W // 4
     dev = masks_in.device
     dsf = torch.empty(max(lt - 1, 1), h, w, 2, device=dev, dtype=torch.float32)
     dsb = torch.empty_like(dsf)
     pmask = torch.empty(lt, h, w, 2, device=dev, dtype=torch.float32)
-    check(_lib.lib().pp_gen_prep(_p(_dense(flows_f)), _p(_dense(flows_b)), _p(_dense(masks_in)), _p(_dense(masks_upd)),
-                                 _p(dsf), _p(dsb), _p(pmask), lt, H, W, _stream()), "pp_gen_prep")
+    if flows_f.dtype == torch.float16:                         # half-precision clip storage, widened in the kernel
+        check(_lib.lib().pp_gen_prep_f16(_p(_dense(flows_f), torch.float16), _p(_dense(flows_b), torch.float16), _p(_dense(masks_in)),
+                                         _p(_dense(masks_upd)), _p(dsf), _p(dsb), _p(pmask), lt, H, W, _stream()), "pp_gen_prep_f16")
+    else:
+        check(_lib.lib().pp_gen_prep(_p(_dense(flows_f)), _p(_dense(flows_b)), _p(_dense(masks_in)), _p(_dense(masks_upd)),
+                                     _p(dsf), _p(dsb), _p(pmask), lt, H, W, _stream()), "pp_gen_prep")
     _count(1)
     return dsf[:lt - 1], dsb[:lt - 1], pmask
 
