@@ -299,12 +299,24 @@ int pp_resize_u8_nearest(const uint8_t* src, uint8_t* dst, int T, int H, int W, 
                          cudaStream_t stream);
 int pp_resize_u8_bilinear_cv(const uint8_t* src, uint8_t* dst, int T, int H, int W, int Ho, int Wo, const int* xofs, const short* alpha,
                              const int* yofs, const short* beta, cudaStream_t stream);
+/* resize_flow (utils/flow_util.py:6-11) of the evaluation dataset (core/dataset.py:213-214): cv2.resize(INTER_LINEAR) of
+ * float32 flows, then component 0 *= float32(Wo/W), component 1 *= float32(Ho/H).  Planar [N][2][H][W] -> [N][2][Ho][Wo].
+ * HOST helper pp_resample_coeffs_linear_f32: OpenCV's float tables for one axis, ofs [out], coef [out*2] = (1-f, f).
+ * Tables are device copies (unused, may be NULL, for the same size and for exact 2x down-scaling, which is OpenCV's
+ * INTER_AREA fast path). */
+int pp_resample_coeffs_linear_f32(int in_size, int out_size, int horizontal, int* ofs, float* coef);
+int pp_resize_flow_linear_cv(const float* src, float* dst, int N, int H, int W, int Ho, int Wo, const int* xofs, const float* alpha,
+                             const int* yofs, const float* beta, cudaStream_t stream);
 #define PP_MAX_WINDOW 32
 typedef struct PPWindowIds { int n; int frame[PP_MAX_WINDOW]; int first[PP_MAX_WINDOW]; } PPWindowIds;
 /* inference_propainter.py:437-450: pred planar [n][3][H][W] in (-1,1), masks planar [T][1][H][W],
  * ori/comp uint8 [T][H][W][3]; ids (host struct): target frame + first-visit flag per local frame. */
 int pp_composite_blend_u8(const float* pred, const float* masks, const uint8_t* ori, uint8_t* comp,
                           const PPWindowIds* ids, int H, int W, cudaStream_t stream);
+/* scripts/evaluate_propainter.py:166-179: the same inputs, but comp is a float32 clip [T][H][W][3]: a first visit stores
+ * the uint8 composite, a later one prev*0.5 + img*0.5 without truncation. */
+int pp_composite_blend_f32(const float* pred, const float* masks, const uint8_t* ori, float* comp,
+                           const PPWindowIds* ids, int H, int W, cudaStream_t stream);
 /* ---- video outpainting (inference_propainter.py --mode video_outpainting) --------------------------- */
 /* extrapolation inference_propainter.py:117-156 + to_tensors of its masks (:265-266): uint8 frames [T][h][w][3] are
  * placed at (top, left) of a zero canvas [T][H][W][3]; flow_masks / masks_dilated float {0,1} [T][1][H][W] are 1 outside

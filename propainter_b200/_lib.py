@@ -128,6 +128,10 @@ SIGNATURES = {
                                          c_void_p]),
     "pp_composite_blend_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(PPWindowIds), c_int, c_int,
                                       c_void_p]),
+    "pp_composite_blend_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(PPWindowIds), c_int, c_int,
+                                       c_void_p]),
+    "pp_resample_coeffs_linear_f32": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p]),
+    "pp_resize_flow_linear_cv": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] * 5),
     "pp_extrapolate_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 9 + [c_void_p]),
     "pp_mask_overlay_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pp_flow_maxrad": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [ctypes.c_float, c_void_p]),

@@ -1117,6 +1117,26 @@ extern "C" int pp_composite_blend_u8(const float* pred, const float* masks, cons
   return PP_OK;
 }
 
+__global__ void __launch_bounds__(256) k_composite_f32(const float* __restrict__ pred, const float* __restrict__ masks,
+    const uint8_t* __restrict__ ori, float* __restrict__ comp, PPWindowIds ids, int H, int W) {
+  long i = (long)blockIdx.x * blockDim.x + threadIdx.x;      // over n*H*W*3 (HWC order of the float32 clip buffer)
+  long HW = (long)H * W;
+  if (i >= (long)ids.n * HW * 3) return;
+  int k = (int)(i / (HW * 3)); long r = i - (long)k * HW * 3; long p = r / 3; int c = (int)(r - p * 3);
+  int idx = ids.frame[k];
+  long o = ((long)idx * HW + p) * 3 + c;
+  comp[o] = pp_composite_f32(pred[((long)k * 3 + c) * HW + p], masks[(long)idx * HW + p], ori[o], comp[o], ids.first[k]);
+}
+// the float-valued compositing / blending of scripts/evaluate_propainter.py:166-179 (the evaluation protocol)
+extern "C" int pp_composite_blend_f32(const float* pred, const float* masks, const uint8_t* ori, float* comp,
+                                      const PPWindowIds* ids, int H, int W, cudaStream_t stream) {
+  if (ids->n < 1 || ids->n > PP_MAX_WINDOW) return PP_ERR_SHAPE;
+  long n = (long)ids->n * H * W * 3;
+  k_composite_f32<<<pp_blocks(n, 256), 256, 0, stream>>>(pred, masks, ori, comp, *ids, H, W);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+
 // ================================================================ video outpainting + masked preview
 // One thread per canvas pixel: its 3 canvas bytes and its value in both masks.  64-bit offsets (a 3840x2160 canvas
 // holds 8.3 M pixels per frame).

@@ -376,14 +376,24 @@ PP_HD float pp_up2_blend(float v00, float v01, float v10, float v11, const PPUp&
 // ------------------------------------------------------------------------------------------------
 // Final compositing (inference_propainter.py:437-450): uint8 truncation, masked composite,
 // order-dependent 1/2-1/2 running blend (truncating again).
-PP_HD uint8_t pp_composite(float pred, float mask, uint8_t ori, uint8_t prev, int first) {
+PP_HD uint8_t pp_composite_img(float pred, float mask, uint8_t ori) {
   float v = PP_MUL(PP_DIV(PP_ADD(pred, 1.0f), 2.0f), 255.0f);
   uint8_t p8 = (uint8_t)(int)v;                     // numpy astype(uint8) of a value in [0,255]
   uint8_t bm = (uint8_t)(int)mask;
-  uint8_t img = (uint8_t)(p8 * bm + ori * (uint8_t)(1 - bm));
+  return (uint8_t)(p8 * bm + ori * (uint8_t)(1 - bm));
+}
+PP_HD uint8_t pp_composite(float pred, float mask, uint8_t ori, uint8_t prev, int first) {
+  uint8_t img = pp_composite_img(pred, mask, ori);
   if (first) return img;
   float b = PP_ADD(PP_MUL((float)prev, 0.5f), PP_MUL((float)img, 0.5f));
   return (uint8_t)(int)b;
+}
+// The evaluation script's compositing (scripts/evaluate_propainter.py:166-179): the same uint8 `img`, but a later visit
+// blends into a float32 frame and is not truncated again, so a frame seen by k windows holds multiples of 2^-(k-1).
+PP_HD float pp_composite_f32(float pred, float mask, uint8_t ori, float prev, int first) {
+  float img = (float)pp_composite_img(pred, mask, ori);
+  if (first) return img;
+  return PP_ADD(PP_MUL(prev, 0.5f), PP_MUL(img, 0.5f));
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -11,7 +11,10 @@
 //     source x = (int)(xo), xo starting at scale/2 and accumulated by += scale in double (Geometry.c) -- table on the host.
 //   * the output cv2.resize(f, out_size) (:469-470): OpenCV's 8-bit INTER_LINEAR: 11-bit fixed-point coefficients from
 //     float fractions, horizontal pass into int, vertical pass ((b0*(S0>>4))>>16 + (b1*(S1>>4))>>16 + 2) >> 2 (resize.cpp).
-// All kernels: uint8 [T][H][W][3] (masks [T][H][W]) in, same layout out; stream-ordered; the caller owns tables + scratch.
+//   * the evaluation dataset's resize_flow (core/dataset.py:213-214, utils/flow_util.py:6-11): OpenCV's float32
+//     INTER_LINEAR (float coefficients, separable, unfused products and sums; exact 2x down-scaling is its INTER_AREA
+//     fast path) and the per-component rescale, on planar float32 flows [N][2][H][W].
+// The uint8 kernels: uint8 [T][H][W][3] (masks [T][H][W]) in, same layout out; stream-ordered; the caller owns tables + scratch.
 #include <math.h>
 #include <stdint.h>
 #include "pp_common.cuh"
@@ -103,6 +106,26 @@ extern "C" int pp_resample_coeffs_linear_cv(int in_size, int out_size, int horiz
     const float c0 = (1.f - f) * 2048.f, c1 = f * 2048.f;
     coef[2 * d] = (short)lrintf(c0);                          // saturate_cast<short>(float): round half to even
     coef[2 * d + 1] = (short)lrintf(c1);
+  }
+  return PP_OK;
+}
+
+// OpenCV INTER_LINEAR tables of the float32 path for one axis: ofs[out] = left / top source index, coef[out*2] =
+// (1 - f, f) in float.  Same coordinate rule as above; the horizontal border reset likewise.
+extern "C" int pp_resample_coeffs_linear_f32(int in_size, int out_size, int horizontal, int* ofs, float* coef) {
+  if (in_size < 1 || out_size < 1 || !ofs || !coef) return PP_ERR_SHAPE;
+  const double inv_scale = (double)out_size / in_size, scale = 1.0 / inv_scale;
+  for (int d = 0; d < out_size; ++d) {
+    float f = (float)((d + 0.5) * scale - 0.5);
+    int s = (int)floorf(f);
+    f -= s;
+    if (horizontal) {
+      if (s < 0) { f = 0; s = 0; }
+      if (s >= in_size - 1) { f = 0; s = in_size - 1; }
+    }
+    ofs[d] = s;
+    coef[2 * d] = 1.f - f;
+    coef[2 * d + 1] = f;
   }
   return PP_OK;
 }
@@ -212,5 +235,53 @@ extern "C" int pp_resize_u8_bilinear_cv(const uint8_t* src, uint8_t* dst, int T,
   if (W == 2 * Wo && H == 2 * Ho) return PP_ERR_SHAPE;
   const long n = (long)T * Ho * Wo;
   k_resize_linear_cv<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(src, dst, T, H, W, Ho, Wo, xofs, alpha, yofs, beta);
+  return cudaPeekAtLastError() == cudaSuccess ? PP_OK : PP_ERR_LAUNCH;
+}
+
+// One output value of resize_flow (utils/flow_util.py:6-11) per thread, planar [N][2][H][W] -> [N][2][Ho][Wo].  Every
+// product and sum is rounded on its own (OpenCV's float kernels are not contracted to FMA on its x86 builds), then the
+// component's in-place `*= new / old` with the ratio already rounded to float32 (numpy's weak Python scalar).
+__device__ __forceinline__ float rs_row_linear(const float* __restrict__ row, int W, int sx, float a0, float a1) {
+  return sx + 1 < W ? PP_ADD(PP_MUL(row[sx], a0), PP_MUL(row[sx + 1], a1)) : PP_MUL(row[sx], a0);   // right border: a0 = 1
+}
+__global__ void __launch_bounds__(256) k_resize_flow_linear(const float* __restrict__ src, float* __restrict__ dst, int N, int H,
+    int W, int Ho, int Wo, const int* __restrict__ xofs, const float* __restrict__ alpha, const int* __restrict__ yofs,
+    const float* __restrict__ beta, float scale_u, float scale_v) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long)N * 2 * Ho * Wo) return;
+  const int x = (int)(i % Wo); const long r = i / Wo; const int y = (int)(r % Ho); const long plane = r / Ho;
+  const float* s = src + plane * H * W;
+  const int sx = xofs[x];
+  const float a0 = alpha[2 * x], a1 = alpha[2 * x + 1];
+  int sy0 = yofs[y], sy1 = sy0 + 1;
+  sy0 = sy0 < 0 ? 0 : (sy0 > H - 1 ? H - 1 : sy0);                    // rows clamp, their weights stay (resize.cpp)
+  sy1 = sy1 < 0 ? 0 : (sy1 > H - 1 ? H - 1 : sy1);
+  const float r0 = rs_row_linear(s + (long)sy0 * W, W, sx, a0, a1), r1 = rs_row_linear(s + (long)sy1 * W, W, sx, a0, a1);
+  const float v = PP_ADD(PP_MUL(r0, beta[2 * y]), PP_MUL(r1, beta[2 * y + 1]));
+  dst[i] = PP_MUL(v, (plane & 1) ? scale_v : scale_u);
+}
+// exact 2x down-scaling on both axes: OpenCV's INTER_AREA fast path, ((a + b) + c) + d over the 2x2 block, times 0.25
+__global__ void __launch_bounds__(256) k_resize_flow_area2(const float* __restrict__ src, float* __restrict__ dst, int N, int H,
+    int W, int Ho, int Wo, float scale_u, float scale_v) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long)N * 2 * Ho * Wo) return;
+  const int x = (int)(i % Wo); const long r = i / Wo; const int y = (int)(r % Ho); const long plane = r / Ho;
+  const float* p = src + (plane * H + 2L * y) * W + 2L * x;
+  const float sum = PP_ADD(PP_ADD(PP_ADD(p[0], p[1]), p[W]), p[W + 1]);
+  dst[i] = PP_MUL(PP_MUL(sum, 0.25f), (plane & 1) ? scale_v : scale_u);
+}
+extern "C" int pp_resize_flow_linear_cv(const float* src, float* dst, int N, int H, int W, int Ho, int Wo, const int* xofs,
+                                        const float* alpha, const int* yofs, const float* beta, cudaStream_t stream) {
+  if (N < 1 || H < 1 || W < 1 || Ho < 1 || Wo < 1) return PP_ERR_SHAPE;
+  const long n = (long)N * 2 * Ho * Wo;
+  const float su = (float)((double)Wo / W), sv = (float)((double)Ho / H);
+  if (Ho == H && Wo == W)                                                // cv2.resize copies; the ratios are 1
+    return cudaMemcpyAsync(dst, src, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, stream) == cudaSuccess ? PP_OK : PP_ERR_LAUNCH;
+  if (W == 2 * Wo && H == 2 * Ho)
+    k_resize_flow_area2<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(src, dst, N, H, W, Ho, Wo, su, sv);
+  else if (!xofs || !alpha || !yofs || !beta)
+    return PP_ERR_SHAPE;
+  else
+    k_resize_flow_linear<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(src, dst, N, H, W, Ho, Wo, xofs, alpha, yofs, beta, su, sv);
   return cudaPeekAtLastError() == cudaSuccess ? PP_OK : PP_ERR_LAUNCH;
 }

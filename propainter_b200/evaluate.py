@@ -25,14 +25,16 @@ import torch.nn.functional as F
 
 
 def psnr_frames(a_u8, b_u8):
-    """[T,H,W,3] uint8 x2 (tensors) -> float64 tensor [T] (inf where identical)"""
+    """[T,H,W,3] uint8 x2 (tensors) -> float64 tensor [T] (inf where identical).  Float frames (the evaluation protocol's
+    blended video) are widened to float64 as they are, as calc_psnr_and_ssim does."""
     d = (a_u8.double() - b_u8.double()) ** 2
     mse = d.flatten(1).mean(1)
     return torch.where(mse == 0, torch.full_like(mse, float("inf")), 20.0 * torch.log10(255.0 / mse.sqrt()))
 
 
 def ssim_frames(a_u8, b_u8, win_size=65, data_range=255.0):
-    """skimage compare_ssim(multichannel=True, win_size=65, data_range=255) per frame: [T,H,W,3] uint8 x2 -> float64 [T]"""
+    """skimage compare_ssim(multichannel=True, win_size=65, data_range=255) per frame: [T,H,W,3] uint8 x2 -> float64 [T]
+    (float frames are taken at their float64 value, as for psnr_frames)"""
     T, H, W, C = a_u8.shape
     if min(H, W) < win_size:
         raise ValueError("win_size exceeds image extent")
@@ -177,3 +179,135 @@ def flow_epe_summary(results):
     epe = sum(n * (r["epe_forward"] + r["epe_backward"]) for n, r in zip(flows, results)) / (2 * sum(flows))
     return {"epe": epe, "seconds_per_frame": sum(r["seconds"] for r in results) / sum(r["frames"] for r in results),
             "videos": len(results)}
+
+
+# ---------------------------------------------------------------- the evaluation script's video-completion protocol
+PROTOCOL_RAFT_CLIP = 60                 # evaluate_propainter.py:108 short_len: RAFT chunks of 60 frames, 1-frame overlap
+
+
+def prepare_test_video(frames_u8, masks_u8, size, flows=None, device="cuda"):
+    """TestDataset.__getitem__ (core/dataset.py:173-231) after file I/O, on the device.  size = (w, h), the script's
+    args.size.  frames_u8 uint8 [T,H0,W0,3] (RGB) -> [T,h,w,3] by cv2.resize(INTER_LINEAR) -- these frames are both the
+    network input and the ground truth; masks_u8 uint8 [T,H0,W0] -> float {0,1} [1,T,1,h,w]: PIL NEAREST resize, > 0,
+    cv2.dilate with the 3x3 cross x4; flows: an optional (forward, backward) pair of float32 [T-1,2,Hf,Wf] -> [T-1,2,h,w]
+    through resize_flow (utils/flow_util.py:6-11).  Returns (frames, masks, flows or None).  An exact 2x down-scaling of
+    the frames, where OpenCV switches the 8-bit resize to INTER_AREA, raises (the uint8 kernel does not implement it)."""
+    from . import ops
+    w, h = (int(s) for s in size)
+    dev = torch.device(device)
+    fr = ops.resize_output_u8(torch.as_tensor(frames_u8).to(dev).contiguous(), (w, h))
+    mk = ops.resize_masks_u8(torch.as_tensor(masks_u8).to(dev).contiguous(), (w, h))
+    mk = ops.mask_dilate(mk, 4).unsqueeze(0)
+    if flows is not None:
+        flows = tuple(ops.resize_flow(torch.as_tensor(f).to(dev).float().contiguous(), (w, h)) for f in flows)
+    return fr, mk, flows
+
+
+@torch.no_grad()
+def evaluate_video(pipe, frames_u8, masks, flows=None, task="video_completion", neighbor_length=20, ref_stride=10,
+                   raft_iter=20, i3d=None, cfg=None):
+    """The per-video body of scripts/evaluate_propainter.py::main_worker (:92-210) on prepare_test_video's outputs:
+    frames_u8 uint8 [T,h,w,3], masks float {0,1} [1,T,1,h,w] (one mask set for flow completion, propagation, the
+    generator and compositing), flows the loaded (forward, backward) pair [T-1,2,h,w] or [1,T-1,2,h,w] (--load_flow),
+    or None: RAFT with `raft_iter` iterations in chunks of 60 frames overlapping by one (:108-124).
+
+    Unlike the inference schedule (ProPainterPipeline.__call__): flow completion and image propagation run once over the
+    whole clip; windows of `neighbor_length` (stride neighbor_length // 2) take every `ref_stride`-th frame of the clip
+    as reference, with no cap; and the composited video stays float32 (ops.composite_blend_f32), a frame seen by several
+    windows holding multiples of 1/2 or 1/4.  `seconds` is the synchronised wall time from after the upload to after
+    compositing (:100-101, :181-184).  video_completion: per-frame PSNR / SSIM in float64 of the float frames against
+    the input frames, and with `i3d` (an InceptionI3d) the pair (real, comp truncated to uint8) of I3D activations.
+    object_removal only times.  `cfg`: an InferenceConfig for what the script leaves open (windows_in_flight); its
+    schedule fields are replaced by the protocol's, and half_storage raises ValueError (the script has no such mode)."""
+    from dataclasses import replace
+    from . import ops
+    from .inference_propainter import InferenceConfig
+    if task not in ("video_completion", "object_removal"):
+        raise ValueError(f"task must be 'video_completion' or 'object_removal', got {task!r}")
+    cfg = cfg or InferenceConfig()
+    if cfg.half_storage:
+        raise ValueError("evaluate_video: the evaluation protocol keeps fp32 clip storage (half_storage is not supported)")
+    dev = pipe.device
+    ori = torch.as_tensor(frames_u8).to(dev).contiguous()
+    T, H, W, _ = ori.shape
+    mk = torch.as_tensor(masks).to(dev).float().reshape(1, T, 1, H, W).contiguous()
+    cfg = replace(cfg, raft_iter=raft_iter, neighbor_length=neighbor_length, ref_stride=ref_stride,
+                  subvideo_length=max(T, 1), raft_clip_frames=PROTOCOL_RAFT_CLIP)
+    frames = ops.u8_to_frames(ori).unsqueeze(0)                  # the dataset's frame_tensors
+    torch.cuda.synchronize(dev)
+    t0 = time.perf_counter()
+    if flows is not None:
+        gt = tuple(torch.as_tensor(f).to(dev).float().reshape(1, T - 1, 2, H, W) for f in flows)
+    else:
+        gt = pipe.compute_flows(frames, cfg)
+    pred = pipe.complete_flows(gt, mk, cfg)                       # subvideo_length >= T: one pass over the clip
+    del gt
+    prop, upd_m = pipe.model.img_propagation(frames * (1 - mk), pred, mk, "nearest")
+    upd_f = frames * (1 - mk) + prop * mk
+    del prop, frames
+    comp = torch.zeros(T, H, W, 3, device=dev, dtype=torch.float32)
+    pipe.generate(upd_f, mk, upd_m, pred, ori, cfg, comp=comp, composite=ops.composite_blend_f32)
+    torch.cuda.synchronize(dev)
+    dt = time.perf_counter() - t0
+    out = {"frames": T, "seconds": dt, "seconds_per_frame": dt / T, "comp": comp}
+    if task == "video_completion":
+        ps, ss = psnr_frames(ori, comp).tolist(), ssim_frames(ori, comp).tolist()
+        out.update(psnr_per_frame=ps, ssim_per_frame=ss, psnr=sum(ps) / len(ps), ssim=sum(ss) / len(ss))
+        if i3d is not None:
+            out["i3d"] = (i3d_activations(i3d, ori), i3d_activations(i3d, comp.to(torch.uint8)))
+    return out
+
+
+def protocol_video_line(index, count, name, rec, avg_psnr, avg_ssim, avg_time):
+    """the per-video line evaluate_propainter.py:219-226 prints and writes (its backslash continuation keeps the next
+    source line's indentation inside the string)"""
+    if "psnr" not in rec:
+        return f'[{index + 1:3}/{count}] Name: {str(name):25} | Time: {avg_time:.4f}'
+    return (f'[{index + 1:3}/{count}] Name: {str(name):25} | PSNR/SSIM: {rec["psnr"]:.4f}/{rec["ssim"]:.4f} '
+            f'                    | Avg PSNR/SSIM: {avg_psnr:.4f}/{avg_ssim:.4f} | Time: {avg_time:.4f}')
+
+
+def evaluate_propainter(pipe, videos, size=(432, 240), task="video_completion", neighbor_length=20, ref_stride=10,
+                        raft_iter=20, i3d=None, cfg=None, log=None):
+    """scripts/evaluate_propainter.py::main_worker's dataset loop over `videos`, an iterable of (name, frames_u8,
+    masks_u8, flows) the caller has read (frames uint8 [T,H0,W0,3] RGB, masks uint8 [T,H0,W0], flows None or the
+    (forward, backward) pair of float32 [T-1,2,Hf,Wf] .flo contents), each prepared by prepare_test_video at
+    size = (w, h) (the script's --width / --height defaults) and scored by evaluate_video.
+
+    Returns {"videos": per-video records (name, psnr / ssim of the video, the running frame averages avg_psnr /
+    avg_ssim, the running mean time per frame avg_time, per-frame metrics, seconds, line = the script's text),
+    "summary": video_completion_summary of the records (PSNR / SSIM over all frames, VFID with `i3d`, mean time per
+    frame), "line": the script's final line}.  `log(text)` receives each line as it is produced.  The composited
+    videos are not kept."""
+    recs = []
+    videos = list(videos)
+    frame_psnr, frame_ssim, times = [], [], []
+    for index, (name, frames_u8, masks_u8, flows) in enumerate(videos):
+        torch.cuda.empty_cache()
+        fr, mk, fl = prepare_test_video(frames_u8, masks_u8, size, flows, pipe.device)
+        r = evaluate_video(pipe, fr, mk, fl, task, neighbor_length, ref_stride, raft_iter, i3d, cfg)
+        r.pop("comp")
+        times.append(r["seconds_per_frame"])
+        avg_time = sum(times) / len(times)
+        r.update(name=name, avg_time=avg_time)
+        if task == "video_completion":
+            frame_psnr += r["psnr_per_frame"]
+            frame_ssim += r["ssim_per_frame"]
+            r.update(avg_psnr=sum(frame_psnr) / len(frame_psnr), avg_ssim=sum(frame_ssim) / len(frame_ssim))
+        r["line"] = protocol_video_line(index, len(videos), name, r, r.get("avg_psnr"), r.get("avg_ssim"), avg_time)
+        if log:
+            log(r["line"])
+        recs.append(r)
+    out = {"videos": recs}
+    if task == "video_completion":
+        s = video_completion_summary(recs)
+        vfid = f'{s["vfid"]:.3f}' if "vfid" in s else "n/a"
+        line = (f'Finish evaluation... Average Frame PSNR/SSIM/VFID: {s["psnr"]:.2f}/{s["ssim"]:.4f}/{vfid} '
+                f'| Time: {s["seconds_per_frame"]:.4f}')
+    else:
+        s = {"seconds_per_frame": sum(times) / len(times), "videos": len(recs)}
+        line = f'Finish evaluation... Time: {s["seconds_per_frame"]:.4f}'
+    out.update(summary=s, line=line)
+    if log:
+        log(line)
+    return out

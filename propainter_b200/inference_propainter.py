@@ -258,7 +258,11 @@ class ProPainterPipeline:
 
     # ---- stage 4 (:406-452)
     def generate(self, upd_frames, masks_dilated, upd_masks, pred_flows, ori_u8, cfg, windows=None, comp=None,
-                 visited=None):
+                 visited=None, composite=None):
+        """`composite(pred, masks, ori_u8, comp, frame_ids, first_flags)` writes a window's prediction into `comp`:
+        ops.composite_blend (uint8, the inference script's) unless given; the evaluation protocol passes
+        ops.composite_blend_f32 with a float32 `comp`."""
+        composite = composite or ops.composite_blend
         T = upd_frames.shape[1]
         plan = window_plan(T, cfg)
         comp = torch.zeros_like(ori_u8) if comp is None else comp
@@ -287,7 +291,7 @@ class ProPainterPipeline:
 
         def consume(k, pred):
             nb = todo[k][1]
-            ops.composite_blend(pred, md, ori_u8, comp, nb, [not visited[i] for i in nb])
+            composite(pred, md, ori_u8, comp, nb, [not visited[i] for i in nb])
             for i in nb:
                 visited[i] = True
         self.run_windows([job(nb, refs) for _, nb, refs in todo], consume, cfg, upd_frames.is_cuda)

@@ -664,6 +664,22 @@ def composite_blend(pred, masks, ori_u8, comp_u8, frame_ids, first_flags):
     _count(1)
 
 
+def composite_blend_f32(pred, masks, ori_u8, comp_f32, frame_ids, first_flags):
+    """The evaluation script's compositing (evaluate_propainter.py:166-179): as composite_blend, but comp is a float32
+    clip [T,H,W,3] (updated in place) and a later visit's 1/2-1/2 blend is not truncated."""
+    if comp_f32.dtype != torch.float32:
+        raise RuntimeError(f"composite_blend_f32: comp must be float32, got {comp_f32.dtype}")
+    n, _, H, W = pred.shape
+    ids = PPWindowIds()
+    ids.n = n
+    for i, (f, fl) in enumerate(zip(frame_ids, first_flags)):
+        ids.frame[i], ids.first[i] = int(f), int(fl)
+    check(_lib.lib().pp_composite_blend_f32(_p(_dense(pred)), _p(_dense(masks)), _p(_dense(ori_u8), torch.uint8),
+                                            _p(_dense(comp_f32)), ctypes.byref(ids), H, W, _stream()),
+          "pp_composite_blend_f32")
+    _count(1)
+
+
 def extrapolate_u8(frames_u8, geometry):
     """extrapolation (inference_propainter.py:117-156) on the device: uint8 [T,h,w,3] and a geometry
     ((H, W), (top, left), (rim_h, rim_w)) from inference_propainter.outpaint_geometry -> (canvas uint8 [T,H,W,3],
@@ -819,6 +835,11 @@ def resample_tables(kind, in_size, out_size, device=None, horizontal=True):
         ofs, coef = torch.empty(out_size, dtype=torch.int32), torch.empty(out_size, 2, dtype=torch.int16)
         check(L.pp_resample_coeffs_linear_cv(in_size, out_size, int(bool(horizontal)), ofs.data_ptr(), coef.data_ptr()), "pp_resample_coeffs_linear_cv")
         res = (ofs, coef)
+    elif kind == "linear_f32":
+        ofs, coef = torch.empty(out_size, dtype=torch.int32), torch.empty(out_size, 2, dtype=torch.float32)
+        check(L.pp_resample_coeffs_linear_f32(in_size, out_size, int(bool(horizontal)), ofs.data_ptr(), coef.data_ptr()),
+              "pp_resample_coeffs_linear_f32")
+        res = (ofs, coef)
     else:
         raise ValueError(kind)
     if device is not None:
@@ -868,5 +889,25 @@ def resize_output_u8(frames_u8, size):
     out = torch.empty(T, Ho, Wo, 3, dtype=torch.uint8, device=dev)
     check(_lib.lib().pp_resize_u8_bilinear_cv(_p(_dense(frames_u8), torch.uint8), _p(out, torch.uint8), T, H, W, Ho, Wo, _p(xo, torch.int32),
                                               _p(xa, torch.int16), _p(yo, torch.int32), _p(ya, torch.int16), _stream()), "pp_resize_u8_bilinear_cv")
+    _count(1)
+    return out
+
+
+def resize_flow(flows, size):
+    """resize_flow (utils/flow_util.py:6-11) as the evaluation dataset applies it to loaded flows (core/dataset.py:213-214):
+    cv2.resize(INTER_LINEAR) of float32 flows, then u *= Wo/W and v *= Ho/H in float32.  Planar [N,2,H,W] -> [N,2,Ho,Wo],
+    size = (Wo, Ho) like cv2."""
+    if flows.dtype != torch.float32 or flows.dim() != 4 or flows.shape[1] != 2:
+        raise ValueError(f"resize_flow: expected float32 flows [N,2,H,W], got {flows.dtype} {tuple(flows.shape)}")
+    N, _, H, W = flows.shape
+    Wo, Ho = (int(s) for s in size)
+    if Wo < 1 or Ho < 1:
+        raise ValueError(f"resize_flow: bad size {size}")
+    dev = flows.device
+    xo, xa = resample_tables("linear_f32", W, Wo, dev, True)
+    yo, ya = resample_tables("linear_f32", H, Ho, dev, False)
+    out = torch.empty(N, 2, Ho, Wo, dtype=torch.float32, device=dev)
+    check(_lib.lib().pp_resize_flow_linear_cv(_p(_dense(flows)), _p(out), N, H, W, Ho, Wo, _p(xo, torch.int32), _p(xa),
+                                              _p(yo, torch.int32), _p(ya), _stream()), "pp_resize_flow_linear_cv")
     _count(1)
     return out
