@@ -195,6 +195,12 @@ int pp_ffn_overlap_add(const float* Y, int ldy, float* Z, int ldz, int frames, i
  * frames = 0 returns PP_OK without a launch. */
 int pp_ffn_overlap_add_f16(const void* Y, int ldy, void* Z, int ldz, int frames, int h, int w, int CH, void* workspace,
                            size_t ws_bytes, cudaStream_t stream);
+/* SoftComp's fold (model/modules/sparse_transformer.py:49-61) after its Linear layer ran as a GEMM into tap-major columns:
+ * cols fp16 [frames*fh*fw][ldc] (column tap*C + c, fh = (h-1)/3+1, fw = (w-1)/3+1, ldc >= 49*C), bmap fp32 [h][w][C] (the
+ * fold of the Linear bias) -> out fp16 [frames][h][w][C].  7x7 / stride 3 / pad 3 overlap-add, fp32 sums in a fixed order,
+ * rounded to nearest once.  8-byte aligned fp16 rows, C % 4 == ldc % 4 == 0 (else PP_ERR_ALIGN); frames = 0 returns PP_OK
+ * without a launch. */
+int pp_sc_fold_f16(const void* cols, long ldc, const float* bmap, void* out, int frames, int h, int w, int C, cudaStream_t stream);
 
 /* ---- transformer glue ------------------------------------------------------------------------ */
 /* SparseWindowAttention.pool_layer (model/modules/sparse_transformer.py:131-133, used :203-206): depthwise Conv2d with
@@ -275,6 +281,9 @@ int pp_instance_norm(const float* x, const float* res, float* out, int n, long H
 /* `deconv` up-sampling, F.interpolate(scale_factor=2, bilinear, align_corners=True)
  * (model/propainter.py:248-253, model/recurrent_flow_completion.py:141-146); pixel-major [n][h][w][C] -> [n][2h][2w][C]. */
 int pp_upsample2x_bilinear(const float* src, float* dst, int n, int h, int w, int C, cudaStream_t stream);
+/* the same on fp16 rows (the half-operand decoder; 16-byte aligned rows, C % 8 == 0, else PP_ERR_ALIGN): blend in fp32, rounded to nearest once.
+ * n = 0 returns PP_OK without a launch. */
+int pp_upsample2x_bilinear_f16(const void* src, void* dst, int n, int h, int w, int C, cudaStream_t stream);
 
 /* ---- driver-side pixel ops (inference_propainter.py) ----------------------------------------- */
 /* read_mask's scipy.ndimage.binary_dilation(mask, iterations=k) (cross structure) + to_tensors (inference_propainter.py:93-107,

@@ -115,6 +115,8 @@ SIGNATURES = {
     "pp_instance_norm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_long, c_int, c_float, c_int, c_int, c_void_p, c_size_t,
                                  c_void_p]),
     "pp_upsample2x_bilinear": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "pp_upsample2x_bilinear_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "pp_sc_fold_f16": (c_int, [c_void_p, c_long, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "pp_mask_dilate": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "pp_u8_to_frames": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pp_resample_coeffs_bicubic": (c_int, [c_int, c_int, c_void_p, c_void_p, c_long]),

@@ -509,6 +509,45 @@ extern "C" int pp_ffn_overlap_add_f16(const void* Y, int ldy, void* Z, int ldz, 
   return pp_ffn_launch((const __half*)Y, ldy, (__half*)Z, ldz, frames, h, w, CH, workspace, ws_bytes, stream);
 }
 
+// ================================================================ SoftComp fold
+// SoftComp's Linear(512 -> 6272) + fold(7x7, stride 3, pad 3) (model/modules/sparse_transformer.py:49-61) as a GEMM into
+// tap-major columns (tap*C + c) followed by this overlap-add: out[f,y,x,c] = sum over the tokens whose 7x7 patch covers
+// (y,x) of cols[token][tap*C + c], in a fixed order (ty, tx descending), plus bmap[y,x,c], the fold of the Linear bias.
+// T = __half: fp16 columns in, fp16 out (sc.bias_conv's operand); the sum is fp32 and rounded once.  No atomics, so the
+// result is the same on every run.
+template <typename T>
+__global__ void __launch_bounds__(256) k_sc_fold(const T* __restrict__ cols, long ldc, const float* __restrict__ bmap, int C,
+                                                 int fh, int fw, int h, int w, T* __restrict__ out) {
+  const int c4n = C >> 2;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;       // over h*w*(C/4) of frame blockIdx.y
+  if (i >= h * w * c4n) return;
+  const int c = (i % c4n) * 4, px = i / c4n, y = px / w, x = px - y * w;
+  const T* cf = cols + (long)blockIdx.y * fh * fw * ldc;
+  float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int ty = (y + 3) / 3, ky; ty >= 0 && (ky = y + 3 - 3 * ty) < 7; --ty) {
+    if (ty >= fh) continue;
+    for (int tx = (x + 3) / 3, kx; tx >= 0 && (kx = x + 3 - 3 * tx) < 7; --tx) {
+      if (tx >= fw) continue;
+      const float4 v = pp_ld4(cf + (long)(ty * fw + tx) * ldc + (ky * 7 + kx) * C + c);
+      s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+    }
+  }
+  const float4 b = *reinterpret_cast<const float4*>(bmap + (long)px * C + c);
+  pp_st4(out + ((long)blockIdx.y * h * w + px) * C + c, make_float4(s.x + b.x, s.y + b.y, s.z + b.z, s.w + b.w));
+}
+// cols: fp16 [frames*fh*fw][ldc], fh = (h-1)/3+1, fw = (w-1)/3+1; bmap fp32 [h][w][C]; out fp16 [frames][h][w][C].
+// frames = 0 returns PP_OK without a launch.
+extern "C" int pp_sc_fold_f16(const void* cols, long ldc, const float* bmap, void* out, int frames, int h, int w, int C,
+                              cudaStream_t stream) {
+  if (frames < 0 || frames > 65535 || h < 1 || w < 1 || C < 4 || ldc < 49L * C || (long)h * w * C > 0x7fffffffL) return PP_ERR_SHAPE;
+  if (C % 4 || ldc % 4 || ((uintptr_t)cols & 7) || ((uintptr_t)out & 7) || ((uintptr_t)bmap & 15)) return PP_ERR_ALIGN;
+  if (frames == 0) return PP_OK;
+  k_sc_fold<__half><<<dim3(pp_blocks((long)h * w * (C / 4), 256), frames), 256, 0, stream>>>(
+      (const __half*)cols, ldc, bmap, C, (h - 1) / 3 + 1, (w - 1) / 3 + 1, h, w, (__half*)out);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+
 // ================================================================ conv epilogue + x2 upsampling
 // out = post(act(x + bias[c]) + res) on pixel-major tensors with explicit pixel strides: one pass instead of cuDNN's
 // separate bias add_ kernel, the activation kernel, the residual add and (with a strided `out`) the torch.cat that
@@ -709,22 +748,28 @@ extern "C" int pp_instance_norm(const float* x, const float* res, float* out, in
   return PP_OK;
 }
 
-__global__ void __launch_bounds__(256) k_upsample2x(const float* __restrict__ src, float* __restrict__ dst, int n, int h,
-                                                    int w, int C) {
-  const int c4n = C >> 2, H = 2 * h, W = 2 * w;
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;  // over n*H*W*(C/4)
-  if (i >= (long)n * H * W * c4n) return;
-  const int c = (int)(i % c4n) * 4; const long px = i / c4n;
+// T = __half (the generator's half-operand decoder): fp16 rows in and out, the blend in fp32, the result rounded once; each
+// thread takes 8 channels (16-byte loads and stores) instead of 4.
+template <typename T>
+__global__ void __launch_bounds__(256) k_upsample2x(const T* __restrict__ src, T* __restrict__ dst, int n, int h, int w, int C) {
+  constexpr int V = 16 / sizeof(T);                            // channels per thread
+  const int cvn = C >> (V == 4 ? 2 : 3), H = 2 * h, W = 2 * w;
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;  // over n*H*W*(C/V)
+  if (i >= (long)n * H * W * cvn) return;
+  const int c = (int)(i % cvn) * V; const long px = i / cvn;
   const int b = (int)(px / ((long)H * W)); const int r = (int)(px - (long)b * H * W); const int y = r / W, x = r - y * W;
   const PPUp uy = pp_up2_coord(y, h), ux = pp_up2_coord(x, w);
-  const float* p = src + (((long)b * h + uy.i0) * w + ux.i0) * C + c;
-  const float4 v00 = *reinterpret_cast<const float4*>(p), v01 = *reinterpret_cast<const float4*>(p + (long)ux.step * C);
-  const float4 v10 = *reinterpret_cast<const float4*>(p + (long)uy.step * w * C);
-  const float4 v11 = *reinterpret_cast<const float4*>(p + ((long)uy.step * w + ux.step) * C);
-  float4 o;
-  o.x = pp_up2_blend(v00.x, v01.x, v10.x, v11.x, uy, ux); o.y = pp_up2_blend(v00.y, v01.y, v10.y, v11.y, uy, ux);
-  o.z = pp_up2_blend(v00.z, v01.z, v10.z, v11.z, uy, ux); o.w = pp_up2_blend(v00.w, v01.w, v10.w, v11.w, uy, ux);
-  reinterpret_cast<float4*>(dst)[i] = o;
+  const T* p = src + (((long)b * h + uy.i0) * w + ux.i0) * C + c;
+#pragma unroll
+  for (int k = 0; k < V; k += 4) {
+    const float4 v00 = pp_ld4(p + k), v01 = pp_ld4(p + (long)ux.step * C + k);
+    const float4 v10 = pp_ld4(p + (long)uy.step * w * C + k);
+    const float4 v11 = pp_ld4(p + ((long)uy.step * w + ux.step) * C + k);
+    float4 o;
+    o.x = pp_up2_blend(v00.x, v01.x, v10.x, v11.x, uy, ux); o.y = pp_up2_blend(v00.y, v01.y, v10.y, v11.y, uy, ux);
+    o.z = pp_up2_blend(v00.z, v01.z, v10.z, v11.z, uy, ux); o.w = pp_up2_blend(v00.w, v01.w, v10.w, v11.w, uy, ux);
+    pp_st4(dst + i * V + k, o);
+  }
 }
 // replaces F.interpolate(scale_factor=2, mode='bilinear', align_corners=True) of `deconv`
 // (model/propainter.py:248-253, model/recurrent_flow_completion.py:141-146); pixel-major in/out
@@ -732,7 +777,17 @@ extern "C" int pp_upsample2x_bilinear(const float* src, float* dst, int n, int h
   if (C % 4) return PP_ERR_ALIGN;
   if (h < 2 || w < 2) return PP_ERR_SHAPE;
   const long total = (long)n * 4 * h * w * (C / 4);
-  k_upsample2x<<<pp_blocks(total, 256), 256, 0, stream>>>(src, dst, n, h, w, C);
+  k_upsample2x<float><<<pp_blocks(total, 256), 256, 0, stream>>>(src, dst, n, h, w, C);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+// the same on fp16 rows (16-byte aligned, C % 8 == 0); n = 0 returns PP_OK without a launch
+extern "C" int pp_upsample2x_bilinear_f16(const void* src, void* dst, int n, int h, int w, int C, cudaStream_t stream) {
+  if (C % 8 || ((uintptr_t)src & 15) || ((uintptr_t)dst & 15)) return PP_ERR_ALIGN;
+  if (n < 0 || h < 2 || w < 2) return PP_ERR_SHAPE;
+  if (n == 0) return PP_OK;
+  const long total = (long)n * 4 * h * w * (C / 8);
+  k_upsample2x<__half><<<pp_blocks(total, 256), 256, 0, stream>>>((const __half*)src, (__half*)dst, n, h, w, C);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }

@@ -15,7 +15,7 @@ the owning ``InpaintGenerator`` (a ParamNet); these helpers only execute.
 import torch
 import torch.nn.functional as F
 
-from ... import config, ops
+from ... import autotune, config, ops
 from ...nn_util import as_nchw, as_pm, cl, conv
 from ...window_index import padded_grid, token_grid, window_key_table
 
@@ -82,20 +82,64 @@ class TransformerExec:
         """fp16 copies of fc1 / fc2 weights and biases"""
         return self.net.packed(f"f16:ffn{i}", lambda: tuple(t.half() for t in self._ffn(i)))
 
+    def _ss_half(self):
+        """fp16 copy of the SoftSplit conv weight; the bias stays fp32"""
+        return self.net.packed("f16:ss", lambda: (self._ss()[0].half(), self._ss()[1]))
+
+    def _sc_half(self):
+        """fp16 SoftComp weights: the transposed-conv weight, and the Linear weight with its output rows tap-major
+        (row tap*C + c; the Linear's own rows are c*49 + tap, fold's channel-major order) for the GEMM + fold plan"""
+        def build():
+            W = self.net.P["sc.embedding.weight"]
+            wcol = W.view(self.channel, KS * KS, self.hidden).transpose(0, 1).reshape(-1, self.hidden)
+            return self._sc().half(), wcol.half().contiguous()
+        return self.net.packed("f16:sc", build)
+
+    def _scbc(self, half):
+        P = self.net.P
+        wb = self.net.packed("scbc", lambda: (cl(P["sc.bias_conv.weight"]), P["sc.bias_conv.bias"].contiguous()))
+        return self.net.packed("f16:scbc", lambda: (wb[0].half(), wb[1])) if half else wb
+
     # ------------------------------------------------------------------ soft split / composition
     def soft_split(self, feat):
-        """feat [t,c,h,w] channels_last -> tokens [t,fh,fw,hidden] pixel-major (SoftSplit.forward :19-31)."""
+        """feat [t,c,h,w] channels_last -> tokens [t,fh,fw,hidden] pixel-major, fp32 (SoftSplit.forward :19-31).  fp16 feat
+        (half-operand trunk): fp16 weight, fp32 accumulation, and the bias is added as the fp16 conv output is widened."""
+        if feat.dtype == torch.float16:
+            t, _, h, w = feat.shape
+            fh, fw = token_grid((h, w))
+            out = torch.empty(t, fh, fw, self.hidden, device=feat.device)
+            conv(feat, self._ss_half(), ST, PD, out=as_nchw(out))
+            return out
         return as_pm(conv(feat, self._ss(), ST, PD))
 
-    def soft_comp(self, tokens, hw, res=None):
-        """tokens [t,fh,fw,hidden] -> [t,c,h,w] (SoftComp.forward :49-61); `res` = skip added in the last conv's epilogue."""
+    def soft_comp(self, tokens, hw, res, frames, half=False, out_dtype=torch.float32):
+        """tokens [t,fh,fw,hidden] -> [frames,c,h,w] for the first `frames` frames (SoftComp.forward :49-61); `res` [frames,c,h,w]
+        = skip added in the last conv's epilogue.  half: fp16 operands with fp32 accumulation -- the Linear + fold as either a
+        fp16 transposed conv or a fp16 GEMM into tap-major columns + pp_sc_fold_f16 (whichever measures faster), then
+        sc.bias_conv on the fp16 result; the output is written in `out_dtype`."""
         fh, fw = tokens.shape[1:3]
-        op = (hw[0] + 2 - 3 * fh, hw[1] + 2 - 3 * fw)
-        y = F.conv_transpose2d(as_nchw(tokens), self._sc(), None, stride=ST, padding=PD, output_padding=op)
-        y = y + self._sc_bias_map(tuple(hw))
-        P = self.net.P
-        return conv(y, self.net.packed("scbc", lambda: (cl(P["sc.bias_conv.weight"]), P["sc.bias_conv.bias"].contiguous())), 1, 1,
-                    res=res)
+        tok = tokens[:frames]
+        bmap = self._sc_bias_map(tuple(hw))
+        if not half:
+            op = (hw[0] + 2 - 3 * fh, hw[1] + 2 - 3 * fw)
+            y = F.conv_transpose2d(as_nchw(tok), self._sc(), None, stride=ST, padding=PD, output_padding=op)
+            y = y + bmap
+        else:
+            tok16 = tok.half()
+            wt, wcol = self._sc_half()
+
+            def tconv(tok16):
+                op = (hw[0] + 2 - 3 * fh, hw[1] + 2 - 3 * fw)
+                y = F.conv_transpose2d(as_nchw(tok16), wt, None, stride=ST, padding=PD, output_padding=op)
+                return torch.add(y, bmap, out=torch.empty_like(y))            # fp32 sum, rounded once to fp16
+
+            def fold(tok16):
+                with config.fp32_reductions():
+                    cols = torch.mm(tok16.view(-1, self.hidden), wcol.t())
+                return as_nchw(ops.sc_fold(cols, as_pm(bmap)[0], frames, hw[0], hw[1]))
+            y = autotune.pick(("sc_half", tuple(tok16.shape), tuple(hw)), (fold, tconv), tok16)
+        out = torch.empty(frames, hw[0], hw[1], self.channel, device=tokens.device, dtype=out_dtype)
+        return conv(y, self._scbc(half), 1, 1, res=res, out=as_nchw(out))
 
     # ------------------------------------------------------------------ transformer
     def run(self, tokens, hw, flags, t_dilation=2):

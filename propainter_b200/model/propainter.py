@@ -114,11 +114,24 @@ class InpaintGenerator(ParamNet):
         return out
 
     def _decoder(self, x):
+        """x [lt,128,h,w] channels_last -> the pre-tanh image [lt,3,4h,4w], fp32.  fp16 x (half-operand trunk): fp16 weights
+        and maps, fp32 accumulation and epilogues; decoder.6 gets a zero fourth output channel so that its bias is added as
+        the fp16 conv output is widened to the fp32 image."""
         L = dict(act="leaky", slope=0.2)
-        x = conv(up2(x), self._wb("decoder.0.conv"), 1, 1, **L)
-        x = conv(x, self._wb("decoder.2"), 1, 1, **L)
-        x = conv(up2(x), self._wb("decoder.4.conv"), 1, 1, **L)
-        return conv(x, self._wb("decoder.6"), 1, 1)
+        if x.dtype != torch.float16:
+            x = conv(up2(x), self._wb("decoder.0.conv"), 1, 1, **L)
+            x = conv(x, self._wb("decoder.2"), 1, 1, **L)
+            x = conv(up2(x), self._wb("decoder.4.conv"), 1, 1, **L)
+            return conv(x, self._wb("decoder.6"), 1, 1)
+        wb16 = lambda k: self.packed("f16:" + k, lambda: (self._wb(k)[0].half(), self._wb(k)[1]))
+        x = conv(up2(x), wb16("decoder.0.conv"), 1, 1, **L)
+        x = conv(x, wb16("decoder.2"), 1, 1, **L)
+        x = conv(up2(x), wb16("decoder.4.conv"), 1, 1, **L)
+        w6, b6 = self.packed("f16:decoder.6", lambda: (cl(F.pad(self.P["decoder.6.weight"], (0, 0, 0, 0, 0, 0, 0, 1))).half(),
+                                                       F.pad(self.P["decoder.6.bias"], (0, 1)).contiguous()))
+        n, _, H, W = x.shape
+        out = torch.empty(n, H, W, 4, device=x.device)
+        return conv(x, (w6, b6), 1, 1, out=as_nchw(out))[:, :3]
 
     # ------------------------------------------------------------------ learnable feature propagation
     def _feat_propagation(self, x, dsf, dsb, pmask, interpolation, gather_gemm=False):
@@ -408,10 +421,26 @@ class InpaintGenerator(ParamNet):
                 return self._feat_propagation_umma(xl, dsf, dsb, pmask)
             return self._feat_propagation(xl, dsf, dsb, pmask, interpolation)
         local = high_priority(scan)
-        enc2 = torch.cat([local, enc[lt:]], 0).contiguous(memory_format=torch.channels_last)
+        # half-operand trunk (config.half_convs): SoftSplit, SoftComp, sc.bias_conv and the decoder take fp16 operands with
+        # fp32 accumulation; the transformer's residual stream and SoftComp's residual (the fp32 scan output) stay fp32
+        half = enc.is_cuda and config.half_convs()
+        if half:
+            t = enc.shape[0]
+            enc2 = torch.empty(t, h, w, enc.shape[1], device=enc.device, dtype=torch.float16)
+            enc2[:lt].copy_(as_pm(local))
+            enc2[lt:].copy_(enc_pm[lt:])
+            enc2 = as_nchw(enc2)
+        else:
+            enc2 = torch.cat([local, enc[lt:]], 0).contiguous(memory_format=torch.channels_last)
         tok_in = self.tx.soft_split(enc2)
         tok = self.tx.run(tok_in, (h, w), flags, t_dilation)
-        enc3 = self.tx.soft_comp(tok, (h, w), res=enc2)                          # trans_feat + enc_feat (:365-366)
-        if parts is not None:
+        # trans_feat + enc_feat (:365-366).  Only the local frames reach the decoder, so SoftComp runs for them alone; the
+        # parity path computes every frame, in fp32, for parts["enc_out"]
+        if parts is None:
+            enc3 = self.tx.soft_comp(tok, (h, w), local, lt, half, torch.float16 if half else torch.float32)
+        else:
+            res = torch.cat([local, enc[lt:]], 0).contiguous(memory_format=torch.channels_last)
+            enc3 = self.tx.soft_comp(tok, (h, w), res, enc.shape[0], half)
             parts.update(prop_feat=local.contiguous(), tokens_in=tok_in, tokens_out=tok, enc_out=enc3.contiguous())
-        return torch.tanh(self._decoder(enc3[:lt])).contiguous()
+            enc3 = enc3[:lt].half() if half else enc3[:lt]
+        return torch.tanh(self._decoder(enc3)).contiguous()

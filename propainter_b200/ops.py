@@ -576,6 +576,23 @@ def bias_act_(x_pm, bias, act="none", slope=0.0):
     return bias_act(x_pm, bias, act, slope)
 
 
+def sc_fold(cols, bmap, frames, h, w, out=None):
+    """SoftComp's fold after its Linear layer: fp16 tap-major columns [frames*fh*fw, 49*C] (column tap*C + c) + the folded
+    Linear bias bmap (fp32 pixel-major [h,w,C]) -> fp16 pixel-major [frames,h,w,C] (7x7 / stride 3 / pad 3 overlap-add, fp32
+    sums in a fixed order)."""
+    C = bmap.shape[-1]
+    fh, fw = (h - 1) // 3 + 1, (w - 1) // 3 + 1
+    if cols.dim() != 2 or cols.shape[0] != frames * fh * fw or cols.stride(1) != 1 or tuple(bmap.shape) != (h, w, C):
+        raise RuntimeError("sc_fold: shape mismatch")
+    out = torch.empty(frames, h, w, C, device=cols.device, dtype=torch.float16) if out is None else out
+    if tuple(out.shape) != (frames, h, w, C):
+        raise RuntimeError("sc_fold: out shape mismatch")
+    check(_lib.lib().pp_sc_fold_f16(_p(cols, torch.float16), cols.stride(0), _p(_dense(bmap)), _p(_dense(out), torch.float16), frames,
+                                    h, w, C, _stream()), "pp_sc_fold_f16")
+    _count(1)
+    return out
+
+
 def pool_depthwise(x_pm, w_taps, bias, kh, kw):
     """depthwise conv, kernel = stride = (kh,kw): x_pm [n,H,W,C] -> [n,H//kh,W//kw,C]; w_taps [kh*kw, C].  fp16 x_pm (the
     half-operand LayerNorm output): fp16 out, weights / bias / sums fp32."""
@@ -624,10 +641,15 @@ def instance_norm(x_pm, relu=False, res=None, post_relu=False, eps=1e-5, out=Non
 
 
 def upsample2x(x_pm):
-    """pixel-major [n,h,w,C] -> [n,2h,2w,C], bilinear, align_corners=True."""
+    """pixel-major [n,h,w,C] -> [n,2h,2w,C], bilinear, align_corners=True.  fp16 x_pm (the half-operand decoder): fp16 out,
+    blended in fp32."""
     n, h, w, C = x_pm.shape
-    out = torch.empty(n, 2 * h, 2 * w, C, device=x_pm.device, dtype=torch.float32)
-    check(_lib.lib().pp_upsample2x_bilinear(_p(_dense(x_pm)), _p(out), n, h, w, C, _stream()), "pp_upsample2x_bilinear")
+    out = torch.empty(n, 2 * h, 2 * w, C, device=x_pm.device, dtype=x_pm.dtype)
+    if x_pm.dtype == torch.float16:
+        check(_lib.lib().pp_upsample2x_bilinear_f16(_p(_dense(x_pm), torch.float16), _p(out, torch.float16), n, h, w, C, _stream()),
+              "pp_upsample2x_bilinear_f16")
+    else:
+        check(_lib.lib().pp_upsample2x_bilinear(_p(_dense(x_pm)), _p(out), n, h, w, C, _stream()), "pp_upsample2x_bilinear")
     _count(1)
     return out
 
