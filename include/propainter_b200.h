@@ -137,12 +137,24 @@ typedef struct PPConvParams {
 int pp_conv2d_umma(const PPConvParams* prm, cudaStream_t stream);
 /* the tiling pp_conv2d_umma will use for `prm` (no launch): pixel tile, output-channel tile, CTA count, dynamic smem */
 int pp_conv2d_umma_plan(const PPConvParams* prm, int* tile_h, int* tile_w, int* bn, int* ctas, int* smem_bytes);
+/* The same convolution on fp16 operands (f16 x f16 products, fp32 accumulate): seg[i].x and w_packed point to fp16 data,
+ * segments ld % 8 == 0 and 16-byte aligned (else PP_ERR_ALIGN); w_packed [Cout][K] fp16 in 64-channel blocks,
+ * K = KH*KW*sum_i roundup64(C_i), k = ((blk*KH + dy)*KW + dx)*64 + c.  bias / pre / res stay fp32 and the epilogue computes
+ * in fp32.  It writes out (fp32, round_tf32 ignored) and / or out16 (fp16 [n*H*W][ld_out16], ld_out16 % 8 == 0, 16-byte
+ * aligned, rounded to nearest once); at least one of them (else PP_ERR_SHAPE). */
+int pp_conv2d_umma_f16(const PPConvParams* prm, void* out16, int ld_out16, cudaStream_t stream);
+/* the tiling pp_conv2d_umma_f16 will use for `prm` (no launch) */
+int pp_conv2d_umma_plan_f16(const PPConvParams* prm, int* tile_h, int* tile_w, int* bn, int* ctas, int* smem_bytes);
 /* Sampling half of torchvision.ops.deform_conv2d for DeformableAlignment / SecondOrderDeformableAlignment (same call
  * sites as pp_deform_align): x [n][H][W][ld_x] (Cin = 128 | 256), o = raw conv_offset output [n*H*W][ld_o >= 432],
  * o_bias [432] | NULL, flow [n*H*W][2] | NULL -> cols [n*H*W][9*Cin] (k*Cin + c), modulated samples rounded to TF32.
  * x2 != NULL: channels [Cin/2, Cin) come from a second map x2 [n][H][W][ld_x2] (x then holds channels [0, Cin/2)). */
 int pp_deform_gather(const float* x, int ld_x, const float* x2, int ld_x2, const float* o, int ld_o, const float* o_bias,
                      const float* flow, float max_res, float* cols, int n, int H, int W, int Cin, cudaStream_t stream);
+/* pp_deform_gather with fp16 cols (16-byte aligned), each column rounded to nearest once: the A operand of the fp16
+ * deformable GEMM (pp_conv2d_umma_f16).  Inputs and sampling arithmetic stay fp32. */
+int pp_deform_gather_f16(const float* x, int ld_x, const float* x2, int ld_x2, const float* o, int ld_o, const float* o_bias,
+                         const float* flow, float max_res, void* cols, int n, int H, int W, int Cin, cudaStream_t stream);
 /* flow_warp (model/modules/flow_loss_utils.py:6-45; bilinear, zeros padding, align_corners=True) of pixel-major feature
  * maps and fbConsistencyCheck (model/propainter.py:22-31), batched: feat [n][h][w][ld_f] (C channels), fprop / fcheck
  * [n][h][w][2] (x,y) -> warped [n][h][w][ld_w] (NULL to skip; feat may then be NULL), aux [n][h][w][ld_a >= 3] receives
@@ -150,6 +162,10 @@ int pp_deform_gather(const float* x, int ld_x, const float* x2, int ld_x2, const
  * BidirectionalPropagation.forward model/propainter.py:146-148 when the concat buffers of pp_prop_cond are not wanted. */
 int pp_flow_warp_fbcheck(const float* feat, int ld_f, const float* fprop, const float* fcheck, float* warped, int ld_w,
                          float* aux, int ld_a, int n, int h, int w, int C, int round_tf32, cudaStream_t stream);
+/* pp_flow_warp_fbcheck with fp16 warped (ld_w % 8 == 0, 16-byte aligned, else PP_ERR_ALIGN), rounded to nearest once: the
+ * operand of the fp16 offset-net conv.  feat, the flows and aux stay fp32. */
+int pp_flow_warp_fbcheck_f16(const float* feat, int ld_f, const float* fprop, const float* fcheck, void* warped, int ld_w,
+                             float* aux, int ld_a, int n, int h, int w, int C, cudaStream_t stream);
 
 /* ---- generator glue ------------------------------------------------------------------------- */
 /* F.interpolate block of InpaintGenerator.forward model/propainter.py:338-342: flows planar

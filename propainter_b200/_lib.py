@@ -74,10 +74,16 @@ SIGNATURES = {
                                 c_int, c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "pp_conv2d_umma": (c_int, [ctypes.POINTER(PPConvParams), c_void_p]),
     "pp_conv2d_umma_plan": (c_int, [ctypes.POINTER(PPConvParams)] + [c_void_p] * 5),
+    "pp_conv2d_umma_f16": (c_int, [ctypes.POINTER(PPConvParams), c_void_p, c_int, c_void_p]),
+    "pp_conv2d_umma_plan_f16": (c_int, [ctypes.POINTER(PPConvParams)] + [c_void_p] * 5),
     "pp_deform_gather": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_float, c_void_p, c_int, c_int,
                                  c_int, c_int, c_void_p]),
     "pp_flow_warp_fbcheck": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                      c_int, c_void_p]),
+    "pp_deform_gather_f16": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_float, c_void_p, c_int,
+                                     c_int, c_int, c_int, c_void_p]),
+    "pp_flow_warp_fbcheck_f16": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int,
+                                         c_int, c_void_p]),
     "pp_gen_prep": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                             c_void_p]),
     "pp_gen_prep_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,

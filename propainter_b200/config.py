@@ -31,6 +31,8 @@ HALF_OPERANDS   RAFT's refinement-loop convs (convc1, convc2, convf2, the motion
                 computing in fp32, and each sublayer's fp16 output enters the fp32 residual stream in the next LayerNorm.
                 This is active only while those Linear layers would run TF32 anyway (LINEAR_TF32 or
                 torch.backends.cuda.matmul.allow_tf32, CUDA tensors), so a strict-fp32 run stays strict.
+                Where cuDNN may use TF32 (half_convs) it also runs the per-step convs of the two recurrent propagation
+                scans (plan 0 of UMMA_CONV) on the fp16 instance of pp_conv2d_umma; their states stay fp32.
                 Environment: PP_HALF_OPERANDS=0|1.
 AUTOTUNE        time numerically equivalent plans of a step once per shape during warm-up and keep the faster
                 (propainter_b200/autotune.py): grouped conv vs per-group dense convs, conv + pp_bias_act vs cuDNN's fused

@@ -19,11 +19,16 @@
 //   * D: fp32 registers of the consumer warpgroups (warpgroup w: pixels 64w .. 64w+63 of the tile, m64nBNk8 per k-step);
 //     TF32 products (weights are pre-rounded to TF32 at pack time; activations written by this kernel are optionally rounded
 //     on store so the next conv's operands are round-to-nearest TF32 too).
+//   * fp16 instance (F16 = true, pp_conv2d_umma_f16): fp16 operands, m64nNk16 f32.f16.f16, fp32 accumulation.  A 128-byte
+//     SW128 row holds 64 halves, so a "block" is 64 channels and every k-step / box / slot has the byte size of the TF32
+//     instance: the pipeline is the same with half as many blocks.  The epilogue arithmetic is fp32 (bias / pre / res read as
+//     fp32); it writes an fp32 `out`, an fp16 `out16` rounded to nearest once, or both from the same registers.
 // Warp roles: warps 0-7 two consumer warpgroups (wgmma issue + epilogue; the second idles on 64-pixel tiles), warp 8 TMA
 // producer.  Two rings: A (one slot per 32-channel block) and B (one slot per (block, dy) = KW taps), mbarrier full/empty
 // pairs; a consumer releases a slot once the wgmma group that read it has retired.  Descriptor encodings: pp_umma.cuh.
 #include <cuda.h>
 #include <stdlib.h>
+#include <type_traits>
 #include "pp_elem.cuh"
 #include "pp_mma.cuh"
 #include "pp_umma.cuh"
@@ -51,6 +56,7 @@ struct alignas(64) CVParams {
   int ld_pre, ld_res, ld_out;
   int act, post_relu, round_tf32;
   float slope;
+  __half* out16; int ld_out16;        // fp16 instance only
 };
 
 __device__ __forceinline__ void cv_expect_tx(uint32_t bar, uint32_t bytes) {
@@ -64,15 +70,22 @@ __device__ __forceinline__ void cv_tma2(uint32_t dst, const CUtensorMap* tm, int
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                ::"r"(dst), "l"(tm), "r"(k), "r"(n), "r"(bar) : "memory");
 }
-template <int BN>
+template <int BN, bool F16>
 __device__ __forceinline__ void cv_mma(float (&d)[BN / 2], uint64_t a, uint64_t b, int scale_d) {
-  if constexpr (BN == 32) wg_mma_ss_n32(d, a, b, scale_d);
-  else if constexpr (BN == 64) wg_mma_ss_n64(d, a, b, scale_d);
-  else wg_mma_ss_n128(d, a, b, scale_d);
+  if constexpr (F16) {
+    if constexpr (BN == 32) wg_mma_ss_n32_f16(d, a, b, scale_d);
+    else if constexpr (BN == 64) wg_mma_ss_n64_f16(d, a, b, scale_d);
+    else wg_mma_ss_n128_f16(d, a, b, scale_d);
+  } else {
+    if constexpr (BN == 32) wg_mma_ss_n32(d, a, b, scale_d);
+    else if constexpr (BN == 64) wg_mma_ss_n64(d, a, b, scale_d);
+    else wg_mma_ss_n128(d, a, b, scale_d);
+  }
 }
 
-template <int BN>
+template <int BN, bool F16>
 __global__ void __launch_bounds__(CV_THREADS, 1) k_conv_umma(const __grid_constant__ CVParams p) {
+  constexpr int CB = F16 ? 64 : 32;                               // channels per 128-byte block
   extern __shared__ __align__(1024) uint8_t cv_raw[];
   uint8_t* base = cv_raw + ((1024u - (ua_smem(cv_raw) & 1023u)) & 1023u);
   const int a_slot_bytes = p.KW * p.a_copy_bytes;
@@ -113,9 +126,9 @@ __global__ void __launch_bounds__(CV_THREADS, 1) k_conv_umma(const __grid_consta
         cv_expect_tx(bar(sa), (uint32_t)a_slot_bytes);
         for (int dx = 0; dx < p.KW; ++dx)
           if (p.kgroup)
-            cv_tma4(ua_smem(sA + sa * a_slot_bytes + dx * p.a_copy_bytes), &p.tmA[seg], (cb * p.KW + dx) * 32, x0, y0, img, bar(sa));
+            cv_tma4(ua_smem(sA + sa * a_slot_bytes + dx * p.a_copy_bytes), &p.tmA[seg], (cb * p.KW + dx) * CB, x0, y0, img, bar(sa));
           else
-            cv_tma4(ua_smem(sA + sa * a_slot_bytes + dx * p.a_copy_bytes), &p.tmA[seg], cb * 32, x0 + dx - p.KW / 2,
+            cv_tma4(ua_smem(sA + sa * a_slot_bytes + dx * p.a_copy_bytes), &p.tmA[seg], cb * CB, x0 + dx - p.KW / 2,
                     y0 - p.KH / 2, img, bar(sa));
       }
       __syncwarp();
@@ -126,7 +139,7 @@ __global__ void __launch_bounds__(CV_THREADS, 1) k_conv_umma(const __grid_consta
           cv_expect_tx(bar(16 + sb), (uint32_t)b_slot_bytes);
           for (int dx = 0; dx < p.KW; ++dx)
             cv_tma2(ua_smem(sB + sb * b_slot_bytes + dx * b_tap_bytes), &p.tmB,
-                    (p.kgroup ? kbase + cb * p.KW + dx : ib * p.KW + dx) * 32, n0, bar(16 + sb));
+                    (p.kgroup ? kbase + cb * p.KW + dx : ib * p.KW + dx) * CB, n0, bar(16 + sb));
         }
         __syncwarp();
       }
@@ -154,12 +167,12 @@ __global__ void __launch_bounds__(CV_THREADS, 1) k_conv_umma(const __grid_consta
       const int ib = blk * p.KH + dy, sb = ib % p.nb;
       ua_bar_wait(bar(16 + sb), (ib / p.nb) & 1);
       const uint64_t b_desc0 = ua_desc(ua_smem(sB + sb * b_slot_bytes));
-      // descriptors advance in their 16-byte address field: +2 per 8-float k-step, + tap / row offsets >> 4
+      // descriptors advance in their 16-byte address field: +2 per 32-byte k-step (8 floats / 16 halves), + tap / row offsets >> 4
       uint64_t ad = a_desc0 + (uint64_t)((dy * p.BW * 128) >> 4), bd = b_desc0;
       wg_fence();
       for (int dx = 0; dx < p.KW; ++dx) {
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) cv_mma<BN>(acc, ad + 2 * ks, bd + 2 * ks, 1);
+        for (int ks = 0; ks < 4; ++ks) cv_mma<BN, F16>(acc, ad + 2 * ks, bd + 2 * ks, 1);
         ad += (uint64_t)(p.a_copy_bytes >> 4); bd += (uint64_t)(b_tap_bytes >> 4);
       }
       wg_commit();
@@ -189,7 +202,7 @@ __global__ void __launch_bounds__(CV_THREADS, 1) k_conv_umma(const __grid_consta
   const float* __restrict__ bias = p.bias;
   const int post_relu = p.post_relu, round_tf32 = p.round_tf32;
   const float slope = p.slope;
-  const float* prow[2]; const float* rrow[2]; float* orow[2];
+  const float* prow[2]; const float* rrow[2]; float* orow[2]; __half* hrow[2];
   bool ok[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -197,7 +210,12 @@ __global__ void __launch_bounds__(CV_THREADS, 1) k_conv_umma(const __grid_consta
     const int y = y0 + r / p.BW, x = x0 + r % p.BW;
     ok[h] = y < p.H && x < p.W;
     const long pix = ok[h] ? ((long)img * p.H + y) * p.W + x : 0;
-    orow[h] = p.out + pix * p.ld_out + n0 + 2 * t;
+    if constexpr (F16) {
+      orow[h] = p.out ? p.out + pix * p.ld_out + n0 + 2 * t : nullptr;
+      hrow[h] = p.out16 ? p.out16 + pix * p.ld_out16 + n0 + 2 * t : nullptr;
+    } else {
+      orow[h] = p.out + pix * p.ld_out + n0 + 2 * t;
+    }
     prow[h] = p.pre ? p.pre + pix * p.ld_pre + n0 + 2 * t : nullptr;
     rrow[h] = p.res ? p.res + pix * p.ld_res + n0 + 2 * t : nullptr;
   }
@@ -218,8 +236,13 @@ __global__ void __launch_bounds__(CV_THREADS, 1) k_conv_umma(const __grid_consta
         a.x = actf(acc[4 * j + 2 * h] + (bv.x + pv.x)) + rv.x;
         a.y = actf(acc[4 * j + 2 * h + 1] + (bv.y + pv.y)) + rv.y;
         if (post_relu) { a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f); }
-        if (round_tf32) { a.x = __uint_as_float(pp_tf32(a.x)); a.y = __uint_as_float(pp_tf32(a.y)); }
-        *reinterpret_cast<float2*>(orow[h] + 8 * j) = a;
+        if constexpr (F16) {
+          if (orow[h]) *reinterpret_cast<float2*>(orow[h] + 8 * j) = a;
+          if (hrow[h]) *reinterpret_cast<__half2*>(hrow[h] + 8 * j) = __float22half2_rn(a);
+        } else {
+          if (round_tf32) { a.x = __uint_as_float(pp_tf32(a.x)); a.y = __uint_as_float(pp_tf32(a.y)); }
+          *reinterpret_cast<float2*>(orow[h] + 8 * j) = a;
+        }
       }
     }
   };
@@ -263,19 +286,21 @@ static PFN_cvEncodeTiled cv_encoder() {
   return cached;
 }
 
-// tile / ring plan shared by the launcher and pp_conv2d_umma_plan (so callers and tests can see what will run)
-static int cv_plan(const PPConvParams* q, CVParams* p, int* smem_bytes) {
+// tile / ring plan shared by the launcher and pp_conv2d_umma_plan (so callers and tests can see what will run).  f16: blocks of
+// 64 channels (128 B of halves); the boxes, slots and per-k-step costs are those of the TF32 instance.
+static int cv_plan(const PPConvParams* q, CVParams* p, int* smem_bytes, bool f16) {
+  const int cb = f16 ? 64 : 32, lda = f16 ? 8 : 4;               // channels per block; ld granule of a 16-byte row stride
   if (q->nseg < 1 || q->nseg > PP_CONV_MAX_SEG || q->n < 1 || q->H < 1 || q->W < 1) return PP_ERR_SHAPE;
   if (q->KH < 1 || q->KW < 1 || q->KH > 7 || q->KW > 7 || !(q->KH & 1) || !(q->KW & 1)) return PP_ERR_SHAPE;
   if (q->Cout < 4 || q->Cout % 4) return PP_ERR_SHAPE;
   int nblk = 0, kblocks = 0;
   for (int s = 0; s < q->nseg; ++s) {
     if (q->seg[s].C < 1) return PP_ERR_SHAPE;
-    if (q->seg[s].ld % 4 || ((uintptr_t)q->seg[s].x & 15)) return PP_ERR_ALIGN;
-    p->seg_kblocks[s] = (q->seg[s].C + 31) / 32;
+    if (q->seg[s].ld % lda || ((uintptr_t)q->seg[s].x & 15)) return PP_ERR_ALIGN;
+    p->seg_kblocks[s] = (q->seg[s].C + cb - 1) / cb;
     kblocks += p->seg_kblocks[s];
   }
-  // 1x1 convs (plain GEMMs over the channels): a pipeline stage of one 32-channel block holds only 4 wgmmas per warpgroup,
+  // 1x1 convs (plain GEMMs over the channels): a pipeline stage of one 128-byte block holds only 4 wgmmas per warpgroup,
   // less work than the fixed cost of a stage (two barrier round trips, a wgmma group commit and wait).  Group 4 consecutive
   // blocks per stage (the tap loop walks channels instead of x-shifts).
   const int kv = (q->KH == 1 && q->KW == 1 && kblocks >= 8) ? 4 : 0;
@@ -306,7 +331,8 @@ static int cv_plan(const PPConvParams* q, CVParams* p, int* smem_bytes) {
   if (tiles > 0x7fffffffL) return PP_ERR_SHAPE;
   // N tile.  Model of one k-step of 8 channels for the CTA's two warpgroups (m64nNk8 each, both operands in shared memory):
   // the tensor cores need ~N cycles (1024 TF32 FMA per cycle per SM) and shared memory delivers the 2 x 2 KB A slices plus
-  // 2 x N x 32 B of B at 128 B per cycle, ~32 + N/2 cycles; the larger bounds the step.  One CTA runs per SM (shared
+  // 2 x N x 32 B of B at 128 B per cycle, ~32 + N/2 cycles; the larger bounds the step.  An fp16 k-step (m64nNk16, 16
+  // channels in the same 32 bytes) costs the same: twice the FMAs at twice the rate (2048 per cycle), the same bytes.  One CTA runs per SM (shared
   // memory), CTAs beyond one per SM run as further waves.  Pick the N that minimises waves x step cost; ties go to the
   // larger tile (fewer re-reads of A from L2).
   int bn = q->bn;
@@ -337,13 +363,14 @@ static int cv_plan(const PPConvParams* q, CVParams* p, int* smem_bytes) {
   p->bias = q->bias; p->pre = q->pre; p->res = q->res; p->out = q->out;
   p->ld_pre = q->ld_pre; p->ld_res = q->ld_res; p->ld_out = q->ld_out;
   p->act = q->act; p->post_relu = q->post_relu; p->round_tf32 = q->round_tf32; p->slope = q->slope;
+  p->out16 = nullptr; p->ld_out16 = 0;
   return PP_OK;
 }
 
-extern "C" int pp_conv2d_umma_plan(const PPConvParams* q, int* tile_h, int* tile_w, int* bn, int* ctas, int* smem_bytes) {
+static int cv_plan_report(const PPConvParams* q, bool f16, int* tile_h, int* tile_w, int* bn, int* ctas, int* smem_bytes) {
   CVParams p;
   int smem = 0;
-  const int rc = cv_plan(q, &p, &smem);
+  const int rc = cv_plan(q, &p, &smem, f16);
   if (rc != PP_OK) return rc;
   if (tile_h) *tile_h = p.BH;
   if (tile_w) *tile_w = p.BW;
@@ -353,39 +380,63 @@ extern "C" int pp_conv2d_umma_plan(const PPConvParams* q, int* tile_h, int* tile
   return PP_OK;
 }
 
-extern "C" int pp_conv2d_umma(const PPConvParams* q, cudaStream_t stream) {
+extern "C" int pp_conv2d_umma_plan(const PPConvParams* q, int* tile_h, int* tile_w, int* bn, int* ctas, int* smem_bytes) {
+  return cv_plan_report(q, false, tile_h, tile_w, bn, ctas, smem_bytes);
+}
+
+extern "C" int pp_conv2d_umma_plan_f16(const PPConvParams* q, int* tile_h, int* tile_w, int* bn, int* ctas, int* smem_bytes) {
+  return cv_plan_report(q, true, tile_h, tile_w, bn, ctas, smem_bytes);
+}
+
+static int cv_run(const PPConvParams* q, __half* out16, int ld_out16, bool f16, cudaStream_t stream) {
   CVParams p;
   int smem = 0;
-  int rc = cv_plan(q, &p, &smem);
+  int rc = cv_plan(q, &p, &smem, f16);
   if (rc != PP_OK) return rc;
+  if (f16) {
+    if (!q->out && !out16) return PP_ERR_SHAPE;
+    if (out16 && (ld_out16 % 8 || ((uintptr_t)out16 & 15))) return PP_ERR_ALIGN;
+    p.out16 = out16; p.ld_out16 = ld_out16;
+  } else if (!q->out) {
+    return PP_ERR_SHAPE;
+  }
+  const int cb = f16 ? 64 : 32, esz = f16 ? 2 : 4;
+  const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   PFN_cvEncodeTiled enc = cv_encoder();
   if (!enc) return PP_ERR_LAUNCH;
   for (int s = 0; s < q->nseg; ++s) {
     const cuuint64_t ld = (cuuint64_t)q->seg[s].ld;
     cuuint64_t dims[4] = {(cuuint64_t)q->seg[s].C, (cuuint64_t)q->W, (cuuint64_t)q->H, (cuuint64_t)q->n};
-    cuuint64_t strides[3] = {ld * 4, ld * 4 * (cuuint64_t)q->W, ld * 4 * (cuuint64_t)q->W * (cuuint64_t)q->H};
-    cuuint32_t box[4] = {32, (cuuint32_t)p.BW, (cuuint32_t)(p.BH + p.KH - 1), 1};
+    cuuint64_t strides[3] = {ld * esz, ld * esz * (cuuint64_t)q->W, ld * esz * (cuuint64_t)q->W * (cuuint64_t)q->H};
+    cuuint32_t box[4] = {(cuuint32_t)cb, (cuuint32_t)p.BW, (cuuint32_t)(p.BH + p.KH - 1), 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    if (enc(&p.tmA[s], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)q->seg[s].x, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    if (enc(&p.tmA[s], dt, 4, (void*)q->seg[s].x, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return PP_ERR_LAUNCH;
   }
   {
-    const cuuint64_t ktot = (cuuint64_t)p.kreal * q->KH * q->KW * 32;
+    const cuuint64_t ktot = (cuuint64_t)p.kreal * q->KH * q->KW * cb;
     cuuint64_t dims[2] = {ktot, (cuuint64_t)q->Cout};
-    cuuint64_t strides[1] = {ktot * 4};
-    cuuint32_t box[2] = {32, (cuuint32_t)p.BN};
+    cuuint64_t strides[1] = {ktot * esz};
+    cuuint32_t box[2] = {(cuuint32_t)cb, (cuuint32_t)p.BN};
     cuuint32_t estr[2] = {1, 1};
-    if (enc(&p.tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)q->w_packed, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    if (enc(&p.tmB, dt, 2, (void*)q->w_packed, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return PP_ERR_LAUNCH;
   }
-  void (*kernel)(const CVParams) = p.BN == 32 ? k_conv_umma<32> : p.BN == 64 ? k_conv_umma<64> : k_conv_umma<128>;
+  void (*kernel)(const CVParams) = f16 ? (p.BN == 32 ? k_conv_umma<32, true> : p.BN == 64 ? k_conv_umma<64, true> : k_conv_umma<128, true>)
+                                        : (p.BN == 32 ? k_conv_umma<32, false> : p.BN == 64 ? k_conv_umma<64, false> : k_conv_umma<128, false>);
   if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CV_SMEM_BUDGET + 2048) != cudaSuccess)
     return PP_ERR_LAUNCH;
   dim3 grid((unsigned)(p.tiles_x * p.tiles_y * p.n), (unsigned)((p.Cout + p.BN - 1) / p.BN));
   if (cv_launch(kernel, grid, dim3(CV_THREADS), (size_t)smem, stream, p) != cudaSuccess) return PP_ERR_LAUNCH;
   return cudaPeekAtLastError() == cudaSuccess ? PP_OK : PP_ERR_LAUNCH;
+}
+
+extern "C" int pp_conv2d_umma(const PPConvParams* q, cudaStream_t stream) { return cv_run(q, nullptr, 0, false, stream); }
+
+extern "C" int pp_conv2d_umma_f16(const PPConvParams* q, void* out16, int ld_out16, cudaStream_t stream) {
+  return cv_run(q, static_cast<__half*>(out16), ld_out16, true, stream);
 }
 
 // ================================================================ deformable sampling -> columns
@@ -394,12 +445,12 @@ extern "C" int pp_conv2d_umma(const PPConvParams* q, cudaStream_t stream) {
 // model/recurrent_flow_completion.py:31-44): decode the raw conv_offset output (max_res*tanh offsets (+ flow.flip),
 // sigmoid modulation), sample x bilinearly at the 9 x 16 positions of every pixel and write the modulated samples as
 // columns cols[p][k*Cin + c] (rounded to TF32: they are the A operand of the GEMM that follows = pp_conv2d_umma with a
-// 1x1 kernel over `cols`).  One warp per pixel: lane <-> (group, half of the group's channels), so per tap a warp reads
+// 1x1 kernel over `cols`; the fp16 instance rounds them to nearest fp16 instead, for pp_conv2d_umma_f16).  One warp per pixel: lane <-> (group, half of the group's channels), so per tap a warp reads
 // 16 positions x 4 corners x 32/64 B and writes one contiguous Cin*4-byte run.
-template <int CPL>   // channels per lane: 4 (Cin = 128) or 8 (Cin = 256)
+template <int CPL, typename TC>   // channels per lane: 4 (Cin = 128) or 8 (Cin = 256); column type float (TF32) or __half
 __global__ void __launch_bounds__(256) k_deform_gather(const float* __restrict__ x, int ld_x, const float* __restrict__ x2, int ld_x2,
     const float* __restrict__ o, int ld_o,
-    const float* __restrict__ obias, const float* __restrict__ flow, float max_res, float* __restrict__ cols, long npix, int H, int W) {
+    const float* __restrict__ obias, const float* __restrict__ flow, float max_res, TC* __restrict__ cols, long npix, int H, int W) {
   // One warp per pixel, lane <-> (offset group g, half of the group's channels).  The 27 offset-net outputs of (pixel, g)
   // are fetched up front, then the 9 taps run in batches of 3 with all 12 (24) corner loads of a batch in flight before
   // the first one is used: the kernel is latency-bound (two dependent memory round trips per tap), so what matters is
@@ -429,7 +480,7 @@ __global__ void __launch_bounds__(256) k_deform_gather(const float* __restrict__
   if (second) { x = x2; ld_x = ld_x2; }
   const int cs = second ? c - CIN / 2 : c;
   const float* xi = x + img * HW * ld_x;
-  float* dst = cols + pix * (9L * CIN) + c;
+  TC* dst = cols + pix * (9L * CIN) + c;
 #pragma unroll
   for (int kb = 0; kb < 9; kb += 3) {
     float wts[3][4];
@@ -462,15 +513,23 @@ __global__ void __launch_bounds__(256) k_deform_gather(const float* __restrict__
           const float w = wts[u][j];
           acc.x += v[u][j][i].x * w; acc.y += v[u][j][i].y * w; acc.z += v[u][j][i].z * w; acc.w += v[u][j][i].w * w;
         }
-        *reinterpret_cast<float4*>(dst + (long)(kb + u) * CIN + 4 * i) =
-            make_float4(__uint_as_float(pp_tf32(acc.x)), __uint_as_float(pp_tf32(acc.y)), __uint_as_float(pp_tf32(acc.z)), __uint_as_float(pp_tf32(acc.w)));
+        if constexpr (std::is_same<TC, __half>::value) {
+          const __half2 lo = __floats2half2_rn(acc.x, acc.y), hi = __floats2half2_rn(acc.z, acc.w);
+          uint2 v;
+          v.x = *reinterpret_cast<const uint32_t*>(&lo); v.y = *reinterpret_cast<const uint32_t*>(&hi);
+          *reinterpret_cast<uint2*>(dst + (long)(kb + u) * CIN + 4 * i) = v;
+        } else {
+          *reinterpret_cast<float4*>(dst + (long)(kb + u) * CIN + 4 * i) =
+              make_float4(__uint_as_float(pp_tf32(acc.x)), __uint_as_float(pp_tf32(acc.y)), __uint_as_float(pp_tf32(acc.z)), __uint_as_float(pp_tf32(acc.w)));
+        }
       }
     }
   }
 }
 
-extern "C" int pp_deform_gather(const float* x, int ld_x, const float* x2, int ld_x2, const float* o, int ld_o, const float* o_bias,
-                                const float* flow, float max_res, float* cols, int n, int H, int W, int Cin, cudaStream_t stream) {
+template <typename TC>
+static int dg_run(const float* x, int ld_x, const float* x2, int ld_x2, const float* o, int ld_o, const float* o_bias, const float* flow,
+                  float max_res, TC* cols, int n, int H, int W, int Cin, cudaStream_t stream) {
   if ((Cin != 128 && Cin != 256) || n < 1 || H < 1 || W < 1) return PP_ERR_SHAPE;
   if (ld_x % 4 || ld_o < 432 || ((uintptr_t)x & 15) || ((uintptr_t)cols & 15)) return PP_ERR_ALIGN;
   if (x2 && (ld_x2 % 4 || ((uintptr_t)x2 & 15))) return PP_ERR_ALIGN;
@@ -479,8 +538,18 @@ extern "C" int pp_deform_gather(const float* x, int ld_x, const float* x2, int l
   const long blocks = (npix + 7) / 8;
   if (blocks > 0x7fffffffL) return PP_ERR_SHAPE;
   cudaError_t e;
-  if (Cin == 128) e = cv_launch(k_deform_gather<4>, dim3((unsigned)blocks), dim3(256), 0, stream, x, ld_x, x2, ld_x2, o, ld_o, o_bias, flow, max_res, cols, npix, H, W);
-  else e = cv_launch(k_deform_gather<8>, dim3((unsigned)blocks), dim3(256), 0, stream, x, ld_x, x2, ld_x2, o, ld_o, o_bias, flow, max_res, cols, npix, H, W);
+  if (Cin == 128) e = cv_launch(k_deform_gather<4, TC>, dim3((unsigned)blocks), dim3(256), 0, stream, x, ld_x, x2, ld_x2, o, ld_o, o_bias, flow, max_res, cols, npix, H, W);
+  else e = cv_launch(k_deform_gather<8, TC>, dim3((unsigned)blocks), dim3(256), 0, stream, x, ld_x, x2, ld_x2, o, ld_o, o_bias, flow, max_res, cols, npix, H, W);
   if (e != cudaSuccess) return PP_ERR_LAUNCH;
   return cudaPeekAtLastError() == cudaSuccess ? PP_OK : PP_ERR_LAUNCH;
+}
+
+extern "C" int pp_deform_gather(const float* x, int ld_x, const float* x2, int ld_x2, const float* o, int ld_o, const float* o_bias,
+                                const float* flow, float max_res, float* cols, int n, int H, int W, int Cin, cudaStream_t stream) {
+  return dg_run(x, ld_x, x2, ld_x2, o, ld_o, o_bias, flow, max_res, cols, n, H, W, Cin, stream);
+}
+
+extern "C" int pp_deform_gather_f16(const float* x, int ld_x, const float* x2, int ld_x2, const float* o, int ld_o, const float* o_bias,
+                                    const float* flow, float max_res, void* cols, int n, int H, int W, int Cin, cudaStream_t stream) {
+  return dg_run(x, ld_x, x2, ld_x2, o, ld_o, o_bias, flow, max_res, static_cast<__half*>(cols), n, H, W, Cin, stream);
 }

@@ -1,6 +1,7 @@
 // HBM/L2-bound gather, stencil and elementwise kernels of the ProPainter hot path (sm_90a).
 // One thread (or one warp) per output element; the per-element rules live in pp_elem.cuh.
 #include <stdlib.h>
+#include <type_traits>
 #include "pp_elem.cuh"
 #include "pp_mma.cuh"
 #include "../../include/propainter_b200.h"
@@ -200,9 +201,11 @@ extern "C" int pp_prop_cond(const float* cur, int ld_cur, const float* prop, int
 // One warp per pixel; every lane derives the sampling position itself from the pixel's flow (two broadcast loads) instead
 // of waiting for lane 0 + shuffles, then gathers the 4 bilinear corners as float4 channel vectors (coalesced 512 B per
 // corner for C = 128).  `aux` (optional) receives (fx, fy, valid): the step-independent condition channels of
-// DeformableAlignment's offset net, so their share of conv_offset.0 can be convolved once per scan.
+// DeformableAlignment's offset net, so their share of conv_offset.0 can be convolved once per scan.  TW = __half: `warped`
+// is stored rounded to nearest fp16 (the operand of the fp16 scan convs); the sampling stays fp32.
+template <typename TW>
 __global__ void __launch_bounds__(256) k_flow_warp(long npix, int h, int w, int C, const float* __restrict__ feat, int ld_f,
-    const float* __restrict__ fprop, const float* __restrict__ fcheck, float* __restrict__ warped, int ld_w,
+    const float* __restrict__ fprop, const float* __restrict__ fcheck, TW* __restrict__ warped, int ld_w,
     float* __restrict__ aux, int ld_a, int round_tf32) {
   asm volatile("griddepcontrol.launch_dependents;");              // programmatic dependent launch (see conv_umma.cu)
   asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -217,14 +220,21 @@ __global__ void __launch_bounds__(256) k_flow_warp(long npix, int h, int w, int 
   const PPTaps t = pp_taps(ix, iy, h, w);
   if (warped) {
     const float* f = feat + img * HW * ld_f;
-    float* o = warped + pix * ld_w;
+    TW* o = warped + pix * ld_w;
     for (int c = lane * 4; c < C; c += 128) {
       float4 v = pp_tap_nhwc4(f, ld_f, w, t, c);
-      if (round_tf32) {
-        v.x = __uint_as_float(pp_tf32(v.x)); v.y = __uint_as_float(pp_tf32(v.y));
-        v.z = __uint_as_float(pp_tf32(v.z)); v.w = __uint_as_float(pp_tf32(v.w));
+      if constexpr (std::is_same<TW, __half>::value) {
+        const __half2 lo = __floats2half2_rn(v.x, v.y), hi = __floats2half2_rn(v.z, v.w);
+        uint2 u;
+        u.x = *reinterpret_cast<const uint32_t*>(&lo); u.y = *reinterpret_cast<const uint32_t*>(&hi);
+        *reinterpret_cast<uint2*>(o + c) = u;
+      } else {
+        if (round_tf32) {
+          v.x = __uint_as_float(pp_tf32(v.x)); v.y = __uint_as_float(pp_tf32(v.y));
+          v.z = __uint_as_float(pp_tf32(v.z)); v.w = __uint_as_float(pp_tf32(v.w));
+        }
+        *reinterpret_cast<float4*>(o + c) = v;
       }
-      *reinterpret_cast<float4*>(o + c) = v;
     }
   }
   if (aux && lane == 0) {
@@ -234,12 +244,12 @@ __global__ void __launch_bounds__(256) k_flow_warp(long npix, int h, int w, int 
   }
 }
 
-// flow_warp (model/modules/flow_loss_utils.py:6-45, bilinear / zeros / align_corners=True) of pixel-major maps and
-// fbConsistencyCheck (model/propainter.py:22-31); see include/propainter_b200.h
-extern "C" int pp_flow_warp_fbcheck(const float* feat, int ld_f, const float* fprop, const float* fcheck, float* warped, int ld_w,
-                                    float* aux, int ld_a, int n, int h, int w, int C, int round_tf32, cudaStream_t stream) {
+template <typename TW>
+static int fw_run(const float* feat, int ld_f, const float* fprop, const float* fcheck, TW* warped, int ld_w, float* aux, int ld_a,
+                  int n, int h, int w, int C, int round_tf32, cudaStream_t stream) {
+  const int lda = sizeof(TW) == 2 ? 8 : 4;                       // fp16 rows: 16-byte row strides (a conv operand)
   if (n < 1 || h < 1 || w < 1 || (!warped && !aux)) return PP_ERR_SHAPE;
-  if (warped && (!feat || C % 4 || ld_f % 4 || ld_w % 4 || ((uintptr_t)feat & 15) || ((uintptr_t)warped & 15))) return PP_ERR_ALIGN;
+  if (warped && (!feat || C % 4 || ld_f % 4 || ld_w % lda || ((uintptr_t)feat & 15) || ((uintptr_t)warped & 15))) return PP_ERR_ALIGN;
   if (aux && (!fcheck || ld_a < 3)) return PP_ERR_SHAPE;
   const long npix = (long)n * h * w;
   cudaLaunchConfig_t cfg = {};
@@ -249,10 +259,22 @@ extern "C" int pp_flow_warp_fbcheck(const float* feat, int ld_f, const float* fp
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   const char* env = getenv("PP_PDL");
   cfg.attrs = attr; cfg.numAttrs = (env && env[0] == '0') ? 0 : 1;
-  if (cudaLaunchKernelEx(&cfg, k_flow_warp, npix, h, w, C, feat, ld_f, fprop, fcheck, warped, ld_w, aux, ld_a, round_tf32) != cudaSuccess)
+  if (cudaLaunchKernelEx(&cfg, k_flow_warp<TW>, npix, h, w, C, feat, ld_f, fprop, fcheck, warped, ld_w, aux, ld_a, round_tf32) != cudaSuccess)
     return PP_ERR_LAUNCH;
   PP_LAUNCH_CHECK();
   return PP_OK;
+}
+
+// flow_warp (model/modules/flow_loss_utils.py:6-45, bilinear / zeros / align_corners=True) of pixel-major maps and
+// fbConsistencyCheck (model/propainter.py:22-31); see include/propainter_b200.h
+extern "C" int pp_flow_warp_fbcheck(const float* feat, int ld_f, const float* fprop, const float* fcheck, float* warped, int ld_w,
+                                    float* aux, int ld_a, int n, int h, int w, int C, int round_tf32, cudaStream_t stream) {
+  return fw_run(feat, ld_f, fprop, fcheck, warped, ld_w, aux, ld_a, n, h, w, C, round_tf32, stream);
+}
+
+extern "C" int pp_flow_warp_fbcheck_f16(const float* feat, int ld_f, const float* fprop, const float* fcheck, void* warped, int ld_w,
+                                        float* aux, int ld_a, int n, int h, int w, int C, cudaStream_t stream) {
+  return fw_run(feat, ld_f, fprop, fcheck, static_cast<__half*>(warped), ld_w, aux, ld_a, n, h, w, C, 0, stream);
 }
 
 // ================================================================ RAFT correlation pyramid + lookup

@@ -77,9 +77,19 @@ __device__ __forceinline__ uint64_t ua_desc_mn(uint32_t saddr, uint32_t lbo) {
   return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)(1024 >> 4) << 32) |
          ((uint64_t)1 << 62);
 }
+__device__ __forceinline__ void wg_mma_ss_n32_f16(float (&d)[16], uint64_t a, uint64_t b, int scale_d) {
+  asm volatile("{ .reg .pred p; setp.ne.b32 p, %18, 0; wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0; }"
+               : WG_D8(0), WG_D8(8)
+               : "l"(a), "l"(b), "r"(scale_d));
+}
 __device__ __forceinline__ void wg_mma_ss_n64_f16(float (&d)[32], uint64_t a, uint64_t b, int scale_d) {
   asm volatile("{ .reg .pred p; setp.ne.b32 p, %34, 0; wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0; }"
                : WG_D8(0), WG_D8(8), WG_D8(16), WG_D8(24)
+               : "l"(a), "l"(b), "r"(scale_d));
+}
+__device__ __forceinline__ void wg_mma_ss_n128_f16(float (&d)[64], uint64_t a, uint64_t b, int scale_d) {
+  asm volatile("{ .reg .pred p; setp.ne.b32 p, %66, 0; wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0; }"
+               : WG_D8(0), WG_D8(8), WG_D8(16), WG_D8(24), WG_D8(32), WG_D8(40), WG_D8(48), WG_D8(56)
                : "l"(a), "l"(b), "r"(scale_d));
 }
 // A from registers (4 x half2 per thread: rows g / g + 8, k 2t..2t+1 / 2t+8..2t+9), B MN-major

@@ -185,12 +185,13 @@ class InpaintGenerator(ParamNet):
         return conv(z, self._wb(fp + "fuse.2"), 1, 1, res=as_nchw(x))
 
     # ---- the same scan on the wgmma conv kernel (config.UMMA_CONV)
-    def _uw(self, key, sel, segs):
-        """packed weight of conv `key` restricted to the input channels `sel` (list of (lo, hi)) split into segments `segs`"""
+    def _uw(self, key, sel, segs, half=False):
+        """packed weight of conv `key` restricted to the input channels `sel` (list of (lo, hi)) split into segments `segs`
+        (half: fp16, for conv_umma_f16)"""
         def build():
             w = self.P[key + ".weight"]
-            return ops.pack_conv_weight(torch.cat([w[:, lo:hi] for lo, hi in sel], 1), segs)
-        return self.packed(f"uw:{key}:{sel}:{segs}", build)
+            return (ops.pack_conv_weight_f16 if half else ops.pack_conv_weight)(torch.cat([w[:, lo:hi] for lo, hi in sel], 1), segs)
+        return self.packed(f"uw{16 if half else ''}:{key}:{sel}:{segs}", build)
 
     def _ub(self, key):
         return self.P[key + ".bias"]
@@ -203,20 +204,26 @@ class InpaintGenerator(ParamNet):
         backbone.0 that see the current frame, the flow / validity / mask channels (all known before the scan starts) are
         convolved once per scan for all frames in one batched launch and enter the step as a pre-activation addend.
         Per step: 1 warp + 4 offset convs + gather + GEMM + 2 backbone convs = 9 launches (before: ~17), K on the critical
-        path 7 x 1152 (before: 2376 + 3 x 1152 + 1152 + 2340 + 1152)."""
+        path 7 x 1152 (before: 2376 + 3 x 1152 + 1152 + 2340 + 1152).
+        Under config.half_convs() the per-step convs take fp16 operands (conv_umma_f16): the warped features, the sampled
+        columns and the conv outputs t1 / t2 / t3 / y are fp16; the state, the aligned features (backbone.2's residual), the
+        hoisted shares, the offset-net output o and all epilogue arithmetic stay fp32 (DESIGN.md §4 "Precision")."""
         lt, h, w, C = x.shape
         dev = x.device
         fp = "feat_prop_module."
         U = ops.conv_umma
+        half = x.is_cuda and config.half_convs()
         aux = torch.zeros(lt, h, w, 8, device=dev)                  # [fx fy valid m0 m1 0 0 0]: step-independent condition channels
         aux[..., 3:5] = pmask
         mpad = torch.zeros(lt, h, w, 4, device=dev)                 # mask as a 16-byte aligned segment
         mpad[..., :2] = pmask
-        warp = torch.empty(1, h, w, C, device=dev)
-        t1, t2, t3, y = (torch.empty(1, h, w, C, device=dev) for _ in range(4))
+        dt = torch.float16 if half else torch.float32                # the per-step A operands
+        warp = torch.empty(1, h, w, C, device=dev, dtype=dt)
+        t1, t2, t3, y = (torch.empty(1, h, w, C, device=dev, dtype=dt) for _ in range(4))
         o = torch.empty(1, h, w, 432, device=dev)
-        cols = torch.empty(1, h, w, 9 * C, device=dev)
+        cols = torch.empty(1, h, w, 9 * C, device=dev, dtype=dt)
         albuf = torch.empty(1, h, w, C, device=dev)
+        al16 = torch.empty(1, h, w, C, device=dev, dtype=dt) if half else None
         src, outs = x, {}
         for name in ("backward_1", "forward_1"):
             bwd = name == "backward_1"
@@ -232,6 +239,11 @@ class InpaintGenerator(ParamNet):
             pre_off = U([src, aux[..., :5]], self._uw(po + "0", ((0, C), (2 * C, 2 * C + 5)), (C, 5)), 3, 3, C, bias=self._ub(po + "0"))
             pre_bb = U([src, mpad[..., :2]], self._uw(pb + "0", ((0, C), (2 * C, 2 * C + 2)), (C, 2)), 3, 3, C, bias=self._ub(pb + "0"))
             dst = torch.empty(lt, h, w, C, device=dev)
+            if half:
+                self._feat_scan_f16(src, dst, order, bwd, dsf, dsb, pre_off, pre_bb, po, pb, name, o, albuf, (warp, t1, t2, t3, y, cols, al16))
+                outs[name] = dst
+                src = dst
+                continue
             dwp = self.packed("dcnu:" + name, lambda: ops.pack_deform_weight_umma(self.P[f"{fp}deform_align.{name}.weight"]))
             dbias = self.P[f"{fp}deform_align.{name}.bias"]
             prev = None
@@ -256,6 +268,32 @@ class InpaintGenerator(ParamNet):
         z = U([outs["backward_1"], outs["forward_1"], mpad[..., :2]], self._uw(fp + "fuse.0", ((0, 2 * C + 2),), (C, C, 2)), 3, 3, C,
               bias=self._ub(fp + "fuse.0"), act="leaky", slope=0.2, round_tf32=True)
         return as_nchw(U([z], self._uw(fp + "fuse.2", ((0, C),), (C,)), 3, 3, C, bias=self._ub(fp + "fuse.2"), res=x))
+
+    def _feat_scan_f16(self, src, dst, order, bwd, dsf, dsb, pre_off, pre_bb, po, pb, name, o, albuf, bufs):
+        """the sequential loop of `_feat_propagation_umma` on fp16 operands; dst (fp32) receives the states"""
+        C = src.shape[-1]
+        fp = "feat_prop_module."
+        H = ops.conv_umma_f16
+        warp16, t1, t2, t3, y16, cols16, al16 = bufs
+        dwp = self.packed("dcnu16:" + name, lambda: ops.pack_deform_weight_umma_f16(self.P[f"{fp}deform_align.{name}.weight"]))
+        dbias = self.P[f"{fp}deform_align.{name}.bias"]
+        prev = None
+        for i, idx in enumerate(order):
+            if i == 0:
+                al = src[idx:idx + 1]                                # feat_prop = feat_current (:141-143)
+                a16 = al.to(torch.float16)
+            else:
+                fprop = (dsf[idx] if bwd else dsb[idx - 1])[None]
+                ops.flow_warp_fbcheck(prev, fprop, warped=warp16)
+                H([warp16], self._uw(po + "0", ((C, 2 * C),), (C,), True), 3, 3, C, pre=pre_off[idx:idx + 1], act="leaky", slope=0.1, out16=t1)
+                H([t1], self._uw(po + "2", ((0, C),), (C,), True), 3, 3, C, bias=self._ub(po + "2"), act="leaky", slope=0.1, out16=t2)
+                H([t2], self._uw(po + "4", ((0, C),), (C,), True), 3, 3, C, bias=self._ub(po + "4"), act="leaky", slope=0.1, out16=t3)
+                H([t3], self._uw(po + "6", ((0, C),), (C,), True), 3, 3, 432, bias=self._ub(po + "6"), out=o)
+                ops.deform_gather(prev, o, fprop, 3.0, cols16)
+                al, a16 = albuf, al16
+                H([cols16], dwp, 1, 1, C, bias=dbias, out=albuf, out16=al16)     # fp32 residual + fp16 operand, one pass
+            H([a16], self._uw(pb + "0", ((C, 2 * C),), (C,), True), 3, 3, C, pre=pre_bb[idx:idx + 1], act="leaky", slope=0.2, out16=y16)
+            prev = H([y16], self._uw(pb + "2", ((0, C),), (C,), True), 3, 3, C, bias=self._ub(pb + "2"), res=al, out=dst[idx:idx + 1])
 
     def _lw(self, key, sel, bias=True):
         """(channels_last conv weight, bias | None) of conv `key` restricted to input channels `sel`: list of (lo, hi) ranges
@@ -407,8 +445,8 @@ class InpaintGenerator(ParamNet):
         xl = enc_pm[:lt]
 
         def scan():
-            if config.UMMA_CONV == "auto":  # four plans of the same scan (all TF32 tensor-core products): keep the fastest for this shape
-                return autotune.pick(("gen_prop", tuple(xl.shape[1:])), (lambda a, b, c, d: self._feat_propagation_umma(a, b, c, d),
+            if config.UMMA_CONV == "auto":  # four plans of the same scan (TF32 products; plan 0 on fp16 operands under half_convs, part of the key): keep the fastest
+                return autotune.pick(("gen_prop", tuple(xl.shape[1:]), config.half_convs()), (lambda a, b, c, d: self._feat_propagation_umma(a, b, c, d),
                                                                           lambda a, b, c, d: self._feat_propagation(a, b, c, d, interpolation),
                                                                           lambda a, b, c, d: self._feat_propagation(a, b, c, d, interpolation, True),
                                                                           lambda a, b, c, d: self._feat_propagation_hoisted(a, b, c, d)),

@@ -120,14 +120,15 @@ class RecurrentFlowCompleteNet(ParamNet):
             results[name] = seq.flip(0) if di == 0 else seq
         return conv(as_nchw(torch.cat([results["backward_"], results["forward_"]], -1)), self._w2d(fp + "fusion"), res=x)
 
-    def _uw(self, key, sel, segs):
-        """packed weight of conv `key` restricted to the input channels `sel` (list of (lo, hi)), split into segments `segs`"""
+    def _uw(self, key, sel, segs, half=False):
+        """packed weight of conv `key` restricted to the input channels `sel` (list of (lo, hi)), split into segments `segs`
+        (half: fp16, for conv_umma_f16)"""
         def build():
             w = self.P[key + ".weight"]
             if w.dim() == 5:
                 w = w[:, :, 0]
-            return ops.pack_conv_weight(torch.cat([w[:, lo:hi] for lo, hi in sel], 1), segs)
-        return self.packed(f"uw:{key}:{sel}:{segs}", build)
+            return (ops.pack_conv_weight_f16 if half else ops.pack_conv_weight)(torch.cat([w[:, lo:hi] for lo, hi in sel], 1), segs)
+        return self.packed(f"uw{16 if half else ''}:{key}:{sel}:{segs}", build)
 
     def _propagate_umma(self, x):
         """`_propagate` on the wgmma conv kernel (config.UMMA_CONV): every conv of the scan is one pp_conv2d_umma launch
@@ -135,18 +136,28 @@ class RecurrentFlowCompleteNet(ParamNet):
         from the history buffer (no torch.cat), the deformable conv is pp_deform_gather (split input) + a 1x1 conv over the
         sampled columns, and the shares of conv_offset.0 / backbone.0 that only see the current frame (and, in the forward
         scan, the finished backward features) are convolved for all frames at once before the scan starts and enter the step
-        as a pre-activation addend (conv is linear in its input channels).  8 launches per step (before: ~17)."""
+        as a pre-activation addend (conv is linear in its input channels).  8 launches per step (before: ~17).
+        Under config.half_convs() the per-step convs take fp16 operands (conv_umma_f16): backbone.2 writes each state in
+        fp32 (hist) and its fp16 image (hist16) in one pass, the deformable GEMM writes the aligned features the same way,
+        and the sampled columns and t1 / t2 / t3 / y are fp16; the states, the hoisted shares, o and the epilogues stay
+        fp32 (DESIGN.md §4 "Precision")."""
         t, c, h, w = x.shape
         dev = x.device
         xs = as_pm(x)                                                         # [t,h,w,128]
         fp = "feat_prop_module."
         U = ops.conv_umma
         P = self.P
-        t1, t2, t3, y = (torch.empty(1, h, w, c, device=dev) for _ in range(4))
+        half = x.is_cuda and config.half_convs()
+        dt = torch.float16 if half else torch.float32                        # the per-step A operands
+        t1, t2, t3, y = (torch.empty(1, h, w, c, device=dev, dtype=dt) for _ in range(4))
         o = torch.empty(1, h, w, 432, device=dev)
-        cols = torch.empty(1, h, w, 9 * 2 * c, device=dev)
+        cols = torch.empty(1, h, w, 9 * 2 * c, device=dev, dtype=dt)
         albuf = torch.empty(1, h, w, c, device=dev)
         zero = torch.zeros(1, h, w, c, device=dev)
+        if half:                                                              # fp16 images of the aligned features and states
+            al16 = torch.empty(1, h, w, c, device=dev, dtype=dt)
+            zero16 = torch.zeros(1, h, w, c, device=dev, dtype=dt)
+            hist16 = torch.zeros(t + 2, h, w, c, device=dev, dtype=dt)       # slots 0,1 = zero states, never written
         results = {}
         for di, name in enumerate(("backward_", "forward_")):
             order = list(range(t))[::-1] if di == 0 else list(range(t))
@@ -157,8 +168,13 @@ class RecurrentFlowCompleteNet(ParamNet):
             k = 1 + di
             hsegs = [xs] + ([results["backward_"]] if di == 1 else [])
             pre_bb = U(hsegs, self._uw(pb + "0", ((0, k * c),), (c,) * k), 3, 3, c, bias=P[pb + "0.bias"])
-            dwp = self.packed("dcnu:" + name, lambda: ops.pack_deform_weight_umma(P[f"{fp}deform_align.{name}.weight"]))
             dbias = P[f"{fp}deform_align.{name}.bias"]
+            if half:
+                self._scan_f16(hist, hist16, order, k, pre_off, pre_bb, po, pb, name, o, albuf, zero, (t1, t2, t3, y, cols, al16, zero16))
+                seq = hist[2:]
+                results[name] = seq.flip(0) if di == 0 else seq
+                continue
+            dwp = self.packed("dcnu:" + name, lambda: ops.pack_deform_weight_umma(P[f"{fp}deform_align.{name}.weight"]))
             for i, idx in enumerate(order):
                 if i > 0:
                     s1, s2 = hist[i + 1:i + 2], hist[i:i + 1]                 # state(i-1), state(i-2)
@@ -179,6 +195,32 @@ class RecurrentFlowCompleteNet(ParamNet):
             results[name] = seq.flip(0) if di == 0 else seq
         return as_nchw(U([results["backward_"], results["forward_"]], self._uw(fp + "fusion", ((0, 2 * c),), (c, c)), 1, 1, c,
                          bias=P[fp + "fusion.bias"], res=xs))
+
+    def _scan_f16(self, hist, hist16, order, k, pre_off, pre_bb, po, pb, name, o, albuf, zero, bufs):
+        """the sequential loop of `_propagate_umma` on fp16 operands: state(i) goes to hist[i + 2] (fp32) and hist16[i + 2]"""
+        c = hist.shape[-1]
+        fp = "feat_prop_module."
+        H = ops.conv_umma_f16
+        P = self.P
+        t1, t2, t3, y, cols, al16, zero16 = bufs
+        dwp = self.packed("dcnu16:" + name, lambda: ops.pack_deform_weight_umma_f16(P[f"{fp}deform_align.{name}.weight"]))
+        dbias = P[f"{fp}deform_align.{name}.bias"]
+        for i, idx in enumerate(order):
+            if i > 0:
+                H([hist16[i + 1:i + 2], hist16[i:i + 1]], self._uw(po + "0", ((0, c), (2 * c, 3 * c)), (c, c), True), 3, 3, c,
+                  pre=pre_off[idx:idx + 1], act="leaky", slope=0.1, out16=t1)
+                H([t1], self._uw(po + "2", ((0, c),), (c,), True), 3, 3, c, bias=P[po + "2.bias"], act="leaky", slope=0.1, out16=t2)
+                H([t2], self._uw(po + "4", ((0, c),), (c,), True), 3, 3, c, bias=P[po + "4.bias"], act="leaky", slope=0.1, out16=t3)
+                H([t3], self._uw(po + "6", ((0, c),), (c,), True), 3, 3, 432, bias=P[po + "6.bias"], out=o)
+                ops.deform_gather(hist[i + 1:i + 2], o, None, 5.0, cols, x2=hist[i:i + 1])
+                H([cols], dwp, 1, 1, c, bias=dbias, out=albuf, out16=al16)
+                al, a16 = albuf, al16
+            else:
+                al, a16 = zero, zero16                                      # step 0 propagates the zero state
+            H([a16], self._uw(pb + "0", ((k * c, (k + 1) * c),), (c,), True), 3, 3, c, pre=pre_bb[idx:idx + 1], act="leaky", slope=0.1,
+              out16=y)
+            H([y], self._uw(pb + "2", ((0, c),), (c,), True), 3, 3, c, bias=P[pb + "2.bias"], res=al, out=hist[i + 2:i + 3],
+              out16=hist16[i + 2:i + 3])
 
     def _lw(self, key, sel, bias=True):
         """(channels_last 2-D conv weight, bias | None) of conv `key` restricted to the input channel ranges `sel`"""
@@ -262,8 +304,8 @@ class RecurrentFlowCompleteNet(ParamNet):
             m = conv(m, self._w2d(f"mid_dilation.{i}"), 1, d, d, act="leaky", slope=0.2)
 
         def scan():
-            if config.UMMA_CONV == "auto":  # five plans of the same scan (all TF32 tensor-core products): keep the fastest for this shape
-                return autotune.pick(("rfc_prop", tuple(m.shape[1:])), (self._propagate_umma, self._propagate, lambda a: self._propagate(a, True),
+            if config.UMMA_CONV == "auto":  # five plans of the same scan (TF32 products; plan 0 on fp16 operands under half_convs, part of the key): keep the fastest
+                return autotune.pick(("rfc_prop", tuple(m.shape[1:]), config.half_convs()), (self._propagate_umma, self._propagate, lambda a: self._propagate(a, True),
                                                                         self._propagate_hoisted, lambda a: self._propagate_hoisted(a, True)),
                                      m, reps=2, graph_timed=True)
             if config.UMMA_CONV == "hoisted":

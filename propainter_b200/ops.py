@@ -244,36 +244,47 @@ def tf32_round(w):
     return ((i + 0x1000) & ~0x1FFF).view(torch.float32)
 
 
-def pack_conv_weight(weight, seg_channels=None):
-    """[Cout,Cin,KH,KW] -> [Cout,K] for pp_conv2d_umma: the input channels are split into the segments `seg_channels`
-    (default: one segment), every segment is zero-padded to 32-channel blocks and K runs ((blk*KH + dy)*KW + dx)*32 + c."""
+def _pack_conv_blocks(weight, seg_channels, cb):
     Cout, Cin, KH, KW = weight.shape
     seg_channels = [Cin] if seg_channels is None else list(seg_channels)
     if sum(seg_channels) != Cin:
         raise RuntimeError("pack_conv_weight: segments do not add up to Cin")
     blocks, c0 = [], 0
     for C in seg_channels:
-        for b in range(0, C, 32):
-            cw = min(32, C - b)
-            blk = weight.new_zeros(Cout, KH, KW, 32)
+        for b in range(0, C, cb):
+            cw = min(cb, C - b)
+            blk = weight.new_zeros(Cout, KH, KW, cb)
             blk[..., :cw] = weight[:, c0 + b:c0 + b + cw].permute(0, 2, 3, 1)
-            blocks.append(blk.reshape(Cout, KH * KW * 32))
+            blocks.append(blk.reshape(Cout, KH * KW * cb))
         c0 += C
-    return tf32_round(torch.cat(blocks, 1).contiguous())
+    return torch.cat(blocks, 1).contiguous()
 
 
-def _pm4(t):
+def pack_conv_weight(weight, seg_channels=None):
+    """[Cout,Cin,KH,KW] -> [Cout,K] for pp_conv2d_umma: the input channels are split into the segments `seg_channels`
+    (default: one segment), every segment is zero-padded to 32-channel blocks and K runs ((blk*KH + dy)*KW + dx)*32 + c."""
+    return tf32_round(_pack_conv_blocks(weight, seg_channels, 32))
+
+
+def pack_conv_weight_f16(weight, seg_channels=None):
+    """pack_conv_weight for pp_conv2d_umma_f16: 64-channel blocks, k = ((blk*KH + dy)*KW + dx)*64 + c, fp16 rounded to nearest
+    from the fp32 weight (not from its TF32 image)."""
+    return _pack_conv_blocks(weight, seg_channels, 64).to(torch.float16)
+
+
+def _pm4(t, dtype=torch.float32):
     """[n,H,W,C] pixel-major view (unit channel stride, dense over n*H*W pixels) -> (ptr, ld)."""
     if t.dim() != 4:
         raise RuntimeError("expected [n,H,W,C]")
-    return _pm(t)
+    return _pm(t, dtype)
 
 
 def _conv_params(segs, KH, KW, Cout, w_packed=None, bias=None, act="none", slope=0.0, pre=None, res=None, post_relu=False,
-                 out=None, round_tf32=False, bn=0, tile_w=0, tile_m=0):
-    """PPConvParams of one pp_conv2d_umma call (see conv_umma).  A segment may also be given as its shape (n, H, W, C):
-    its pointer is then null and its ld is C rounded up to a multiple of 4 (the narrowest buffer conv_umma accepts), which
-    is enough for pp_conv2d_umma_plan."""
+                 out=None, round_tf32=False, bn=0, tile_w=0, tile_m=0, half=False):
+    """PPConvParams of one pp_conv2d_umma call (see conv_umma; half: of pp_conv2d_umma_f16, fp16 segments and weight in
+    64-channel blocks).  A segment may also be given as its shape (n, H, W, C): its pointer is then null and its ld is C
+    rounded up to the narrowest row conv_umma accepts (4 floats, 8 halves), which is enough for pp_conv2d_umma_plan."""
+    cb, lda, dt = (64, 8, torch.float16) if half else (32, 4, torch.float32)
     if not 1 <= len(segs) <= _lib.PP_CONV_MAX_SEG:
         raise RuntimeError(f"conv_umma: {len(segs)} input segments (1 to {_lib.PP_CONV_MAX_SEG} supported)")
     shapes = [tuple(s.shape) if isinstance(s, torch.Tensor) else tuple(s) for s in segs]
@@ -284,13 +295,13 @@ def _conv_params(segs, KH, KW, Cout, w_packed=None, bias=None, act="none", slope
     for i, (sgm, shp) in enumerate(zip(segs, shapes)):
         if len(shp) != 4 or shp[:3] != (n, H, W):
             raise RuntimeError("conv_umma: segment shape mismatch")
-        ptr, ld = _pm4(sgm) if isinstance(sgm, torch.Tensor) else (ctypes.c_void_p(None), (shp[3] + 3) // 4 * 4)
+        ptr, ld = _pm4(sgm, dt) if isinstance(sgm, torch.Tensor) else (ctypes.c_void_p(None), (shp[3] + lda - 1) // lda * lda)
         prm.seg[i].x, prm.seg[i].ld, prm.seg[i].C = ptr.value, ld, shp[3]
-        kblocks += (shp[3] + 31) // 32
-    if w_packed is not None and tuple(w_packed.shape) != (Cout, kblocks * KH * KW * 32):
-        raise RuntimeError(f"conv_umma: packed weight {tuple(w_packed.shape)} does not match {(Cout, kblocks * KH * KW * 32)}")
+        kblocks += (shp[3] + cb - 1) // cb
+    if w_packed is not None and tuple(w_packed.shape) != (Cout, kblocks * KH * KW * cb):
+        raise RuntimeError(f"conv_umma: packed weight {tuple(w_packed.shape)} does not match {(Cout, kblocks * KH * KW * cb)}")
     prm.n, prm.H, prm.W, prm.KH, prm.KW = n, H, W, KH, KW
-    prm.w_packed, prm.Cout = _p(_dense(w_packed)).value if w_packed is not None else None, Cout
+    prm.w_packed, prm.Cout = _p(_dense(w_packed), dt).value if w_packed is not None else None, Cout
     prm.bias = _p(bias).value if bias is not None else None
     for name, t in (("pre", pre), ("res", res), ("out", out)):
         if t is None:
@@ -321,23 +332,43 @@ def conv_umma(segs, w_packed, KH, KW, Cout, bias=None, act="none", slope=0.0, pr
     return out
 
 
+def conv_umma_f16(segs, w_packed, KH, KW, Cout, bias=None, act="none", slope=0.0, pre=None, res=None, post_relu=False, out=None,
+                  out16=None, bn=0, tile_w=0, tile_m=0):
+    """conv_umma on fp16 operands (pp_conv2d_umma_f16): segs fp16 [n,H,W,C_i] views, w_packed from pack_conv_weight_f16;
+    bias / pre / res fp32, fp32 accumulation and epilogue.  Writes the fp32 `out` and / or the fp16 `out16` (rounded to
+    nearest once; both from one pass when both are given; neither: a new out16).  Returns out16, else out."""
+    if out is None and out16 is None:
+        n, H, W, _ = segs[0].shape
+        out16 = torch.empty(n, H, W, Cout, device=segs[0].device, dtype=torch.float16)
+    prm = _conv_params(segs, KH, KW, Cout, w_packed, bias, act, slope, pre, res, post_relu, out, False, bn, tile_w, tile_m, half=True)
+    p16, ld16 = (None, 0)
+    if out16 is not None:
+        if tuple(out16.shape) != (prm.n, prm.H, prm.W, Cout):
+            raise RuntimeError(f"conv_umma_f16: out16 shape {tuple(out16.shape)} != {(prm.n, prm.H, prm.W, Cout)}")
+        p16, ld16 = _pm4(out16, torch.float16)
+    check(_lib.lib().pp_conv2d_umma_f16(ctypes.byref(prm), p16, ld16, _stream()), "pp_conv2d_umma_f16")
+    _count(1)
+    return out16 if out16 is not None else out
+
+
 ConvPlan = collections.namedtuple("ConvPlan", "tile_h tile_w bn ctas smem_bytes")
 
 
-def conv_plan(segs, KH, KW, Cout, bn=0, tile_w=0, tile_m=0, out=None, pre=None, res=None, bias=None):
-    """The tile / ring plan conv_umma would launch for these arguments (pp_conv2d_umma_plan), without launching it:
-    ConvPlan(tile_h, tile_w, bn, ctas, smem_bytes).  segs as in conv_umma, or their shapes (n, H, W, C_i).  Raises where
-    conv_umma would refuse the plan."""
-    prm = _conv_params(segs, KH, KW, Cout, bias=bias, pre=pre, res=res, out=out, bn=bn, tile_w=tile_w, tile_m=tile_m)
+def conv_plan(segs, KH, KW, Cout, bn=0, tile_w=0, tile_m=0, out=None, pre=None, res=None, bias=None, half=False):
+    """The tile / ring plan conv_umma (half: conv_umma_f16) would launch for these arguments (pp_conv2d_umma_plan[_f16]),
+    without launching it: ConvPlan(tile_h, tile_w, bn, ctas, smem_bytes).  segs as in conv_umma, or their shapes
+    (n, H, W, C_i).  Raises where conv_umma would refuse the plan."""
+    prm = _conv_params(segs, KH, KW, Cout, bias=bias, pre=pre, res=res, out=out, bn=bn, tile_w=tile_w, tile_m=tile_m, half=half)
     vals = [ctypes.c_int(0) for _ in range(5)]
-    check(_lib.lib().pp_conv2d_umma_plan(ctypes.byref(prm), *[ctypes.byref(v) for v in vals]), "pp_conv2d_umma_plan")
+    fn = _lib.lib().pp_conv2d_umma_plan_f16 if half else _lib.lib().pp_conv2d_umma_plan
+    check(fn(ctypes.byref(prm), *[ctypes.byref(v) for v in vals]), "pp_conv2d_umma_plan")
     return ConvPlan(*[v.value for v in vals])
 
 
 def deform_gather(x, o, flow, max_res, cols=None, o_bias=None, x2=None):
     """x [n,H,W,Cin] view (or, with x2, the two halves x | x2 of Cin/2 channels each), o [n,H,W,>=432] raw conv_offset
-    output, flow [n,H,W,2] | None -> cols [n,H,W,9*Cin] (modulated bilinear samples, k*Cin + c, TF32-rounded): the A
-    operand of the deformable conv's GEMM."""
+    output, flow [n,H,W,2] | None -> cols [n,H,W,9*Cin] (modulated bilinear samples, k*Cin + c, TF32-rounded; an fp16 `cols`
+    receives them rounded to nearest fp16): the A operand of the deformable conv's GEMM."""
     n, H, W, Cin = x.shape
     xp, ldx = _pm4(x)
     x2p, ldx2 = (None, 0)
@@ -349,30 +380,39 @@ def deform_gather(x, o, flow, max_res, cols=None, o_bias=None, x2=None):
     op, ldo = _pm4(o)
     if cols is None:
         cols = torch.empty(n, H, W, 9 * Cin, device=x.device, dtype=torch.float32)
-    check(_lib.lib().pp_deform_gather(xp, ldx, x2p, ldx2, op, ldo, _p(o_bias), _p(_dense(flow)) if flow is not None else None,
-                                      float(max_res), _p(_dense(cols)), n, H, W, Cin, _stream()), "pp_deform_gather")
+    fn = _lib.lib().pp_deform_gather_f16 if cols.dtype == torch.float16 else _lib.lib().pp_deform_gather
+    check(fn(xp, ldx, x2p, ldx2, op, ldo, _p(o_bias), _p(_dense(flow)) if flow is not None else None, float(max_res),
+             _p(_dense(cols), cols.dtype), n, H, W, Cin, _stream()), "pp_deform_gather")
     _count(1)
     return cols
 
 
 def flow_warp_fbcheck(feat, fprop, fcheck=None, warped=None, aux=None, want_warp=True, round_tf32=False):
     """flow_warp (bilinear) of pixel-major maps feat [n,h,w,C] by fprop [n,h,w,2] -> warped [n,h,w,C] (views allowed);
-    with fcheck also the forward-backward validity: aux [n,h,w,>=3] view receives (fx, fy, valid).  Returns (warped, aux)."""
+    with fcheck also the forward-backward validity: aux [n,h,w,>=3] view receives (fx, fy, valid).  An fp16 `warped` receives
+    the samples rounded to nearest fp16 (round_tf32 does not apply).  Returns (warped, aux)."""
     n, h, w = fprop.shape[:3]
     fp_, ldf, wp_, ldw, C = None, 0, None, 0, 0
+    f16 = False
     if want_warp:
         C = feat.shape[-1]
         if warped is None:
             warped = torch.empty(n, h, w, C, device=feat.device, dtype=torch.float32)
+        f16 = warped.dtype == torch.float16
         fp_, ldf = _pm4(feat)
-        wp_, ldw = _pm4(warped)
+        wp_, ldw = _pm4(warped, warped.dtype)
     ap, lda = (None, 0)
     if fcheck is not None:
         if aux is None:
             aux = torch.empty(n, h, w, 4, device=fprop.device, dtype=torch.float32)
         ap, lda = _pm4(aux)
-    check(_lib.lib().pp_flow_warp_fbcheck(fp_, ldf, _p(_dense(fprop)), _p(_dense(fcheck)) if fcheck is not None else None, wp_, ldw,
-                                          ap, lda, n, h, w, C, int(bool(round_tf32)), _stream()), "pp_flow_warp_fbcheck")
+    fc = _p(_dense(fcheck)) if fcheck is not None else None
+    if f16:
+        check(_lib.lib().pp_flow_warp_fbcheck_f16(fp_, ldf, _p(_dense(fprop)), fc, wp_, ldw, ap, lda, n, h, w, C, _stream()),
+              "pp_flow_warp_fbcheck_f16")
+    else:
+        check(_lib.lib().pp_flow_warp_fbcheck(fp_, ldf, _p(_dense(fprop)), fc, wp_, ldw, ap, lda, n, h, w, C, int(bool(round_tf32)),
+                                              _stream()), "pp_flow_warp_fbcheck")
     _count(1)
     return warped, aux
 
@@ -381,6 +421,12 @@ def pack_deform_weight_umma(weight):
     """deform-conv weight [Cout,Cin,3,3] -> [Cout, 9*Cin] with k = tap*Cin + c (the column order of deform_gather), TF32."""
     co, ci = weight.shape[:2]
     return tf32_round(weight.permute(0, 2, 3, 1).reshape(co, 9 * ci).contiguous())
+
+
+def pack_deform_weight_umma_f16(weight):
+    """pack_deform_weight_umma for conv_umma_f16 over fp16 columns: [Cout, 9*Cin], k = tap*Cin + c, rounded to nearest fp16."""
+    co, ci = weight.shape[:2]
+    return weight.permute(0, 2, 3, 1).reshape(co, 9 * ci).to(torch.float16).contiguous()
 
 
 def pack_deform_weight(weight):
