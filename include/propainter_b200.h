@@ -30,7 +30,8 @@ const char* pp_error_string(int code);
 int pp_corr_build(const float* fmap, int D, const int* idx1, const int* idx2, int n_pairs, float* lvl0, int h, int w,
                   cudaStream_t stream);
 /* CorrBlock.__init__ :25-27 (3x avg_pool2d).  levels[l]: [planes][h>>l][roundup4(w>>l)] (host array of
- * 4 device pointers); level 0 must be filled. */
+ * 4 device pointers); level 0 must be filled.  Columns w>>l .. roundup4(w>>l)-1 of each row are padding: no entry point
+ * of this section reads or writes them, so the levels may come from any allocation, zeroed or not. */
 int pp_corr_pool_pyramid(float* const* levels, long planes, int h, int w, cudaStream_t stream);
 /* CorrBlock.__call__ :29-50 + bilinear_sampler RAFT/utils/utils.py:57-71.
  * coords [n_pairs*h*w][2] (x,y) -> out pixel-major [n_pairs*h*w][324].  n_pairs = 0 returns PP_OK without a launch. */
@@ -289,7 +290,8 @@ int pp_bias_act_f16(const void* x, int ld_x, int x_f16, const float* bias, const
                     void* out, int ld_out, int out_f16, long n_pix, int C, int act, float slope, int post_relu, cudaStream_t stream);
 
 /* nn.InstanceNorm2d(affine=False, eps) of the RAFT feature encoder (RAFT/extractor.py:18-21,125,168-192) on channels-last
- * maps x [n][HW][C]: out = post(relu?((x - mean) * rstd) + res), statistics per (sample, channel), biased variance.
+ * maps x [n][HW][C]: out = post(relu?((x - mean) * rstd) + res), statistics per (sample, channel), biased variance,
+ * computed from double sums of x minus the channel's value at pixel 0 (no cancellation when |mean| >> std).
  * res nullable (dense, same shape); out may alias x. */
 size_t pp_instance_norm_workspace_bytes(int n, long HW, int C);
 int pp_instance_norm(const float* x, const float* res, float* out, int n, long HW, int C, float eps, int relu, int post_relu,

@@ -134,8 +134,10 @@ static int corr_lookup_tma(const float* const* levels, const float* coords, TO* 
   CUtensorMap tm[4];
   int hl = h, wl = w;
   for (int l = 0; l < 4; ++l) {
+    // x extent wl, not the row stride ld: columns wl..ld-1 are row padding, which the TMA unit must zero-fill like any
+    // other column outside the level (a tap's right corner at x = wl weighs wx1, and the padding is never written)
     const int ld = pp_corr_ld(wl);
-    cuuint64_t dims[3] = {(cuuint64_t)ld, (cuuint64_t)hl, (cuuint64_t)npix};
+    cuuint64_t dims[3] = {(cuuint64_t)wl, (cuuint64_t)hl, (cuuint64_t)npix};
     cuuint64_t strides[2] = {(cuuint64_t)ld * 4, (cuuint64_t)hl * ld * 4};
     cuuint32_t box[3] = {LkGeom<R>::BOXW, LkGeom<R>::BOX, 1};
     cuuint32_t estr[3] = {1, 1, 1};

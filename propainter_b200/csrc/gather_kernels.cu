@@ -675,85 +675,71 @@ extern "C" int pp_bias_act_f16(const void* x, int ld_x, int x_f16, const float* 
 
 // ================================================================ InstanceNorm (RAFT feature encoder)
 // RAFT/extractor.py:18-21,125 (nn.InstanceNorm2d, affine=False, eps 1e-5) on channels-last maps [n][HW][C]:
-// per (sample, channel) biased mean / variance over HW.  Pass 1 writes per-chunk partial sums, pass 2 folds them
-// (in double) and applies (x-mean)*rstd, the ReLU that always follows, and optionally the block's residual add + ReLU.
-// 3 passes over the map (2 reads, 1 write) instead of F.instance_norm's NHWC->NCHW copy, batch_norm and copy back.
-static int pp_in_splits(int n, long HW) {
-  int s = (592 + n - 1) / n;                      // ~4 CTAs per SM over the whole batch
-  if (s > 64) s = 64;
-  if ((long)s * 16 > HW) s = (int)((HW + 15) / 16);
-  return s < 1 ? 1 : s;
-}
+// per (sample, channel) biased mean / variance over HW.  Pass 1 writes per-chunk partial sums of the pivot-shifted values
+// in double (pp_inorm_acc) and the pivots; pass 2 folds them (pp_inorm_fold) and applies (x-mean)*rstd, the ReLU that
+// always follows, and optionally the block's residual add + ReLU.  3 passes over the map (2 reads, 1 write) instead of
+// F.instance_norm's NHWC->NCHW copy, batch_norm and copy back.  The pivots are copied to the workspace so that pass 2 may
+// overwrite pixel 0 in place.
 __global__ void __launch_bounds__(256) k_inorm_stats(const float* __restrict__ x, long HW, int C, int chunk, int S,
-                                                     float* __restrict__ part) {
-  __shared__ float4 sa[256], sb[256];
+                                                     double* __restrict__ part, float* __restrict__ pivot) {
+  __shared__ double sh[8][256];
   const int c4n = C >> 2, R = 256 / c4n;
   const int q = threadIdx.x % c4n, r = threadIdx.x / c4n;
   const long n = blockIdx.y; const int s = blockIdx.x;
   const long r0 = (long)s * chunk; const long r1 = r0 + chunk < HW ? r0 + chunk : HW;
-  float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
+  const float4 p = *reinterpret_cast<const float4*>(x + n * HW * C + 4 * q);
+  double a[4] = {0.0, 0.0, 0.0, 0.0}, b[4] = {0.0, 0.0, 0.0, 0.0};
   if (r < R)
     for (long row = r0 + r; row < r1; row += R) {
       const float4 v = *reinterpret_cast<const float4*>(x + (n * HW + row) * C + 4 * q);
-      a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
-      b.x += v.x * v.x; b.y += v.y * v.y; b.z += v.z * v.z; b.w += v.w * v.w;
+      pp_inorm_acc(a[0], b[0], v.x, p.x); pp_inorm_acc(a[1], b[1], v.y, p.y);
+      pp_inorm_acc(a[2], b[2], v.z, p.z); pp_inorm_acc(a[3], b[3], v.w, p.w);
     }
-  sa[threadIdx.x] = a; sb[threadIdx.x] = b;
+#pragma unroll
+  for (int e = 0; e < 4; ++e) { sh[e][threadIdx.x] = a[e]; sh[4 + e][threadIdx.x] = b[e]; }
   __syncthreads();
   if (r == 0) {
-    for (int j = 1; j < R; ++j) {
-      const float4 u = sa[j * c4n + q], w = sb[j * c4n + q];
-      a.x += u.x; a.y += u.y; a.z += u.z; a.w += u.w;
-      b.x += w.x; b.y += w.y; b.z += w.z; b.w += w.w;
-    }
-    float* dst = part + ((n * S + s) * 2) * C + 4 * q;
-    *reinterpret_cast<float4*>(dst) = a;
-    *reinterpret_cast<float4*>(dst + C) = b;
+    for (int j = 1; j < R; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) { a[e] += sh[e][j * c4n + q]; b[e] += sh[4 + e][j * c4n + q]; }
+    double* dst = part + ((n * S + s) * 2) * C + 4 * q;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) { dst[e] = a[e]; dst[C + e] = b[e]; }
+    if (s == 0) *reinterpret_cast<float4*>(pivot + n * C + 4 * q) = p;
   }
 }
-__global__ void __launch_bounds__(256) k_inorm_apply(const float* x, const float* __restrict__ part, int S, const float* res,
-                                                     float* out, long HW, int C, int chunk, float eps, int relu, int post_relu) {
-  __shared__ float s_mean[512], s_rstd[512];
+__global__ void __launch_bounds__(256) k_inorm_apply(const float* x, const double* __restrict__ part, const float* __restrict__ pivot,
+                                                     int S, const float* res, float* out, long HW, int C, int chunk, float eps,
+                                                     int relu, int post_relu) {
+  __shared__ PPNormStat s_st[512];
   const long n = blockIdx.y; const int s = blockIdx.x;
   for (int c = threadIdx.x; c < C; c += 256) {
     double su = 0.0, sq = 0.0;
     for (int j = 0; j < S; ++j) {
-      su += (double)part[((n * S + j) * 2) * C + c];
-      sq += (double)part[((n * S + j) * 2 + 1) * C + c];
+      su += part[((n * S + j) * 2) * C + c];
+      sq += part[((n * S + j) * 2 + 1) * C + c];
     }
-    const double mean = su / (double)HW;
-    double var = sq / (double)HW - mean * mean;
-    if (var < 0.0) var = 0.0;
-    s_mean[c] = (float)mean;
-    s_rstd[c] = (float)(1.0 / sqrt(var + (double)eps));
+    s_st[c] = pp_inorm_fold(su, sq, HW, pivot[n * C + c], eps);
   }
   __syncthreads();
   const int c4n = C >> 2, R = 256 / c4n;
   const int q = threadIdx.x % c4n, r = threadIdx.x / c4n;
   if (r >= R) return;
-  const float4 m = *reinterpret_cast<const float4*>(s_mean + 4 * q), k = *reinterpret_cast<const float4*>(s_rstd + 4 * q);
   const long r0 = (long)s * chunk; const long r1 = r0 + chunk < HW ? r0 + chunk : HW;
   for (long row = r0 + r; row < r1; row += R) {
     const long off = (n * HW + row) * C + 4 * q;
     const float4 v = *reinterpret_cast<const float4*>(x + off);
-    float y[4] = {(v.x - m.x) * k.x, (v.y - m.y) * k.y, (v.z - m.z) * k.z, (v.w - m.w) * k.w};
-    if (relu) {
+    const float4 t = res ? *reinterpret_cast<const float4*>(res + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float vx[4] = {v.x, v.y, v.z, v.w}, tx[4] = {t.x, t.y, t.z, t.w};
+    float y[4];
 #pragma unroll
-      for (int e = 0; e < 4; ++e) y[e] = fmaxf(y[e], 0.f);
-    }
-    if (res != nullptr) {
-      const float4 t = *reinterpret_cast<const float4*>(res + off);
-      y[0] += t.x; y[1] += t.y; y[2] += t.z; y[3] += t.w;
-    }
-    if (post_relu) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) y[e] = fmaxf(y[e], 0.f);
-    }
+    for (int e = 0; e < 4; ++e) y[e] = pp_inorm_out(vx[e], s_st[4 * q + e], relu, res ? &tx[e] : nullptr, post_relu);
     *reinterpret_cast<float4*>(out + off) = make_float4(y[0], y[1], y[2], y[3]);
   }
 }
+// workspace: n*S*2*C double partial sums, then n*C float pivots
 extern "C" size_t pp_instance_norm_workspace_bytes(int n, long HW, int C) {
-  return (size_t)n * pp_in_splits(n, HW) * 2 * C * sizeof(float);
+  return (size_t)n * pp_inorm_splits(n, HW) * 2 * C * sizeof(double) + (size_t)n * C * sizeof(float);
 }
 // replaces F.instance_norm (+ F.relu, + the residual `relu(x + y)` of ResidualBlock.forward extractor.py:49-57)
 extern "C" int pp_instance_norm(const float* x, const float* res, float* out, int n, long HW, int C, float eps, int relu,
@@ -761,11 +747,12 @@ extern "C" int pp_instance_norm(const float* x, const float* res, float* out, in
   if (C % 4 || ((uintptr_t)x & 15) || ((uintptr_t)out & 15) || ((uintptr_t)res & 15) || ((uintptr_t)workspace & 15)) return PP_ERR_ALIGN;
   if (C < 4 || C > 512 || n < 1 || n > 65535 || HW < 1) return PP_ERR_SHAPE;
   if (ws_bytes < pp_instance_norm_workspace_bytes(n, HW, C)) return PP_ERR_WORKSPACE;
-  const int S = pp_in_splits(n, HW);
+  const int S = pp_inorm_splits(n, HW);
   const int chunk = (int)((HW + S - 1) / S);
-  float* part = (float*)workspace;
-  k_inorm_stats<<<dim3(S, n), 256, 0, stream>>>(x, HW, C, chunk, S, part);
-  k_inorm_apply<<<dim3(S, n), 256, 0, stream>>>(x, part, S, res, out, HW, C, chunk, eps, relu, post_relu);
+  double* part = (double*)workspace;
+  float* pivot = (float*)(part + (size_t)n * S * 2 * C);
+  k_inorm_stats<<<dim3(S, n), 256, 0, stream>>>(x, HW, C, chunk, S, part, pivot);
+  k_inorm_apply<<<dim3(S, n), 256, 0, stream>>>(x, part, pivot, S, res, out, HW, C, chunk, eps, relu, post_relu);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }

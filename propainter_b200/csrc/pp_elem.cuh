@@ -326,6 +326,43 @@ PP_HD float2 pp_convex_up(const float* mask_px, float mask_scale, const float* f
 }
 
 // ------------------------------------------------------------------------------------------------
+// InstanceNorm statistics (nn.InstanceNorm2d, affine=False; k_inorm_stats / k_inorm_apply of gather_kernels.cu).  Each
+// (sample, channel) is shifted by its value at pixel 0, p, and the sums of d = x - p and d^2 are kept in double: d and
+// d^2 of fp32 inputs are exact in double, so the variance E[d^2] - E[d]^2 does not cancel the way E[x^2] - mean^2 in
+// fp32 does when |mean| >> std, and a constant channel gives d = 0, mean = p exactly and 0 out.
+// Splits of the pixel range per sample: ~4 CTAs per SM over the whole batch, >= 16 rows each.
+PP_HD int pp_inorm_splits(int n, long HW) {
+  int s = (592 + n - 1) / n;
+  if (s > 64) s = 64;
+  if ((long)s * 16 > HW) s = (int)((HW + 15) / 16);
+  return s < 1 ? 1 : s;
+}
+PP_HD void pp_inorm_acc(double& s, double& q, float x, float p) {
+  const double d = (double)x - (double)p;
+  s += d;
+  q += d * d;
+}
+struct PPNormStat { float mean, rstd; };
+// the sums over all HW pixels -> fp32 mean and 1/sqrt(biased var + eps), each rounded once from double
+PP_HD PPNormStat pp_inorm_fold(double s, double q, long HW, float p, float eps) {
+  const double md = s / (double)HW;
+  double var = q / (double)HW - md * md;
+  if (var < 0.0) var = 0.0;
+  PPNormStat r;
+  r.mean = (float)((double)p + md);
+  r.rstd = (float)(1.0 / sqrt(var + (double)eps));
+  return r;
+}
+// one output: (x - mean) * rstd, then the optional ReLU, residual add and ReLU of ResidualBlock (extractor.py:49-57)
+PP_HD float pp_inorm_out(float x, const PPNormStat& st, int relu, const float* res, int post_relu) {
+  float y = PP_MUL(PP_SUB(x, st.mean), st.rstd);
+  if (relu) y = fmaxf(y, 0.f);
+  if (res) y = PP_ADD(y, *res);
+  if (post_relu) y = fmaxf(y, 0.f);
+  return y;
+}
+
+// ------------------------------------------------------------------------------------------------
 // InpaintGenerator.forward down-sampling (propainter.py:338-342; stencils pinned in SURVEY.md §8c):
 // bilinear 1/4 (align_corners=False) == mean of the centre 2x2 of each 4x4 block; then /4.
 // The flow plane is fp32 or fp16 clip storage (widened on load).

@@ -82,6 +82,65 @@ void hs_corr_lookup(const float* l0, const float* l1, const float* l2, const flo
   }
 }
 
+// k_corr_lookup<R> (radius 3 or 4): levels [npix][h>>l][roundup4(w>>l)], coords [npix][2] -> out [npix][4K^2]
+void hs_corr_lookup_r(const float* l0, const float* l1, const float* l2, const float* l3, int radius, const float* coords,
+                      float* out, long npix, int h, int w) {
+  const float* lv[4] = {l0, l1, l2, l3};
+  const int K = 2 * radius + 1;
+  for (long pix = 0; pix < npix; ++pix) {
+    int hl = h, wl = w;
+    for (int l = 0; l < 4; ++l) {
+      const int ld = pp_corr_ld(wl);
+      const float* pl = lv[l] + pix * (long)hl * ld;
+      for (int t = 0; t < K * K; ++t)
+        out[pix * 4 * K * K + l * K * K + t] =
+            radius == 3 ? pp_corr_tap_r<3>(pl, hl, wl, ld, coords[2 * pix], coords[2 * pix + 1], l, t / K, t % K)
+                        : pp_corr_tap_r<4>(pl, hl, wl, ld, coords[2 * pix], coords[2 * pix + 1], l, t / K, t % K);
+      hl >>= 1; wl >>= 1;
+    }
+  }
+}
+
+// the on-the-fly tile rule of one level (k_corr_lookup_otf): tile [T*T] (T = 2R+2) at the origin pp_corr_tile_origin_r
+// of (cx, cy) -> out [K*K]; origin [2] receives (tx0, ty0)
+void hs_corr_tap_tile_r(const float* tile, int radius, int hl, int wl, float cx, float cy, int lvl, float* out, int* origin) {
+  const int K = 2 * radius + 1;
+  const int tx0 = radius == 3 ? pp_corr_tile_origin_r<3>(cx, lvl) : pp_corr_tile_origin_r<4>(cx, lvl);
+  const int ty0 = radius == 3 ? pp_corr_tile_origin_r<3>(cy, lvl) : pp_corr_tile_origin_r<4>(cy, lvl);
+  origin[0] = tx0; origin[1] = ty0;
+  for (int t = 0; t < K * K; ++t)
+    out[t] = radius == 3 ? pp_corr_tap_tile_r<3>(tile, tx0, ty0, hl, wl, cx, cy, lvl, t / K, t % K)
+                         : pp_corr_tap_tile_r<4>(tile, tx0, ty0, hl, wl, cx, cy, lvl, t / K, t % K);
+}
+
+// pp_instance_norm on x [n][HW][C]: the statistics rules in k_inorm_stats' split of the rows (S chunks, R row-threads
+// per chunk, merged in thread order), then pp_inorm_fold and pp_inorm_out; res nullable
+void hs_instance_norm(const float* x, const float* res, float* out, int n, long HW, int C, float eps, int relu, int post_relu) {
+  const int S = pp_inorm_splits(n, HW), chunk = (int)((HW + S - 1) / S), R = 256 / (C / 4);
+  std::vector<PPNormStat> st((size_t)C);
+  for (long b = 0; b < n; ++b) {
+    const float* xb = x + b * HW * C;
+    for (int c = 0; c < C; ++c) {
+      double su = 0.0, sq = 0.0;
+      for (int s = 0; s < S; ++s) {
+        const long r0 = (long)s * chunk, r1 = r0 + chunk < HW ? r0 + chunk : HW;
+        double a = 0.0, q = 0.0;
+        for (int r = 0; r < R; ++r) {
+          double ta = 0.0, tq = 0.0;
+          for (long row = r0 + r; row < r1; row += R) pp_inorm_acc(ta, tq, xb[row * C + c], xb[c]);
+          a += ta; q += tq;
+        }
+        su += a; sq += q;
+      }
+      st[c] = pp_inorm_fold(su, sq, HW, xb[c], eps);
+    }
+    for (long i = 0; i < HW * C; ++i) {
+      const long o = b * HW * C + i;
+      out[o] = pp_inorm_out(x[o], st[i % C], relu, res ? res + o : nullptr, post_relu);
+    }
+  }
+}
+
 void hs_convex_upsample(const float* mask, int ld_mask, float scale, const float* flow_lr, float* out, int n, int h, int w) {
   const long H = 8L * h, W = 8L * w;
   for (int b = 0; b < n; ++b)

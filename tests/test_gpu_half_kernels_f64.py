@@ -24,6 +24,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import ops_ref, pipeline_ref
+from tests.raft_front_ref import lookup64, lookup_coords, planes64
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -210,83 +211,6 @@ def _with_subnormals(gen, shape, scale, frac=0.1):
 
 
 # ----------------------------------------------------------------------------------------------- correlation lookup
-def grid_sample_coord32(c, lvl, size):
-    """the plain-load kernel's sampling coordinate (pp_corr_tap_r): c / 2^lvl + (a - 4) for the 9 taps a, through
-    grid_sample's align_corners=True normalise / unnormalise round trip, every step one IEEE fp32 operation (numpy);
-    c [P] fp32 -> [P, 9] float64"""
-    f = np.float32
-    x = c.cpu().numpy().astype(f)[:, None] / f(2 ** lvl) + np.arange(-4, 5, dtype=f)[None, :]
-    g = (f(2) * x) / f(size - 1) - f(1)
-    return torch.from_numpy((((g + f(1)) / f(2)) * f(size - 1)).astype(np.float64)).to(c.device)
-
-
-def lookup64(planes, coords, grid_sample32=False):
-    """float64 CorrBlock lookup (oracle/ops_ref.corr_lookup without its final .float()): planes = 4 float64 levels
-    [P, hl, wl], coords [..., 2] (x, y) with P pixels -> (taps [P, 324], s [P, 324] = sum of |weight * corner|).  Channel
-    l*81 + a*9 + b samples (x + a - 4, y + b - 4) at level l (the reference's window-axis quirk).  The TMA kernel samples
-    at these exact coordinates; the plain-load kernel follows grid_sample's fp32 coordinate round trip
-    (grid_sample32=True), which can move a sample by a few fp32 ulps of the coordinate."""
-    P = planes[0].shape[0]
-    c = coords.reshape(P, 2).double()
-    d = torch.arange(-4, 5, dtype=torch.float64, device=c.device)
-    outs, mags = [], []
-    for l, pl in enumerate(planes):
-        hl, wl = pl.shape[1:]
-        if grid_sample32:
-            x = grid_sample_coord32(coords.reshape(P, 2)[:, 0], l, wl)[:, :, None].expand(P, 9, 9)
-            y = grid_sample_coord32(coords.reshape(P, 2)[:, 1], l, hl)[:, None, :].expand(P, 9, 9)
-        else:
-            x = (c[:, 0, None, None] / 2 ** l + d[None, :, None]).expand(P, 9, 9)
-            y = (c[:, 1, None, None] / 2 ** l + d[None, None, :]).expand(P, 9, 9)
-        x0, y0 = x.floor(), y.floor()
-        fx, fy = x - x0, y - y0
-        flat = pl.reshape(P, -1)
-        o, m = 0, 0
-        for dx, dy, wgt in ((0, 0, (1 - fx) * (1 - fy)), (1, 0, fx * (1 - fy)), (0, 1, (1 - fx) * fy), (1, 1, fx * fy)):
-            xi, yi = x0 + dx, y0 + dy
-            ok = (xi >= 0) & (xi <= wl - 1) & (yi >= 0) & (yi <= hl - 1)
-            idx = (yi.clamp(0, hl - 1) * wl + xi.clamp(0, wl - 1)).long().reshape(P, 81)
-            v = torch.where(ok, torch.gather(flat, 1, idx).view(P, 9, 9), 0.0)
-            o = o + wgt * v
-            m = m + (wgt * v).abs()
-        outs.append(o.reshape(P, 81))
-        mags.append(m.reshape(P, 81))
-    return torch.cat(outs, 1), torch.cat(mags, 1)
-
-
-def planes64(levels, h, w, pairs=None):
-    """the device pyramid (row-padded planes) as float64 [P, hl, wl], optionally only the pixels of `pairs`"""
-    out, hl, wl = [], h, w
-    for lv in levels:
-        v = lv if pairs is None else torch.cat([lv[p * h * w:(p + 1) * h * w] for p in pairs])
-        out.append(v[:, :, :wl].double())
-        hl, wl = hl // 2, wl // 2
-    return out
-
-
-def lookup_coords(B, h, w, seed):
-    """per pixel, by index mod 6: uniform +-6 px around the grid, exact integers, half-integers at level (i // 6) % 4,
-    the borders (x = w-1, y = h-1, -0.5), centres 500 px outside (all-zero windows), uniform +-20 px"""
-    gen = _gen(seed)
-    ys, xs = torch.meshgrid(torch.arange(h, device=DEV), torch.arange(w, device=DEV), indexing="ij")
-    base = torch.stack([xs, ys], -1).double()[None].expand(B, h, w, 2).reshape(-1, 2)
-    n = base.shape[0]
-    i = torch.arange(n, device=DEV)
-    kind, sub = (i % 6)[:, None], (i // 6)
-    uni = lambda r: (torch.rand(n, 2, generator=gen, device=DEV, dtype=torch.float64) * 2 - 1) * r
-    ints = base + torch.randint(-6, 7, (n, 2), generator=gen, device=DEV)
-    lvl = (2.0 ** (sub % 4)).double()[:, None]
-    halves = ((base / lvl).floor() + torch.randint(-3, 4, (n, 2), generator=gen, device=DEV) + 0.5) * lvl
-    bx = torch.stack([torch.tensor([w - 1.0, -0.5, w - 1.0, -0.5], device=DEV)[sub % 4],
-                      torch.tensor([h - 1.0, -0.5, -0.5, h - 1.0], device=DEV)[(sub // 4) % 4]], 1).double()
-    border = torch.where(torch.rand(n, 2, generator=gen, device=DEV) < 0.75, bx, base + uni(3))
-    far = base + torch.where((sub % 2 == 0)[:, None], 500.0, -500.0)
-    c = torch.where(kind == 0, base + uni(6), base + uni(20))
-    for k, v in ((1, ints), (2, halves), (3, border), (4, far)):
-        c = torch.where(kind == k, v, c)
-    return c.float().view(B, h, w, 2), (kind == 4).view(B, h, w)
-
-
 def _pyramid(B, h, w, seed, frames=None):
     """the 4-level device pyramid of B pairs of random 256-channel feature maps (consecutive frames, both directions)"""
     from propainter_b200 import ops
