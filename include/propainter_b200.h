@@ -309,6 +309,11 @@ int pp_upsample2x_bilinear_f16(const void* src, void* dst, int n, int h, int w, 
 int pp_mask_dilate(const uint8_t* src, float* dst, int T, int H, int W, int iterations, cudaStream_t stream);
 /* to_tensors()(frames)*2-1  core/utils.py:130-170 + inference_propainter.py:264: uint8 [T][H][W][3] -> planar float */
 int pp_u8_to_frames(const uint8_t* src, float* dst, int T, int H, int W, cudaStream_t stream);
+/* scripts/compute_flow.py:67-92 (its frame preparation before RAFT): ToTensor (v / 255), F.interpolate(size=(h, w),
+ * mode='bilinear', align_corners=False) and img*2 - 1, fused: uint8 RGB [T][H0][W0][3] -> planar float [T][3][h][w] in [-1,1],
+ * equal to ATen's CPU resize bit for bit (pp_resize_coord in csrc/pp_elem.cuh); at h == H0, w == W0 equal to
+ * pp_u8_to_frames.  Any size < 1: PP_ERR_SHAPE. */
+int pp_u8_to_frames_resized(const uint8_t* src, float* dst, int T, int H0, int W0, int h, int w, cudaStream_t stream);
 /* ---- resizing around the path (inference_propainter.py:34-45 resize_frames, :95-96 mask resize, :469-470 output resize) --- */
 /* HOST helpers (no GPU work): the per-axis tables of the three library resamplers the reference calls.
  * bicubic: Pillow's Image.resize(size) on 8-bit images (BICUBIC, 22-bit fixed point): bounds [out*2] = (first source index,

@@ -125,6 +125,7 @@ SIGNATURES = {
     "pp_sc_fold_f16": (c_int, [c_void_p, c_long, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "pp_mask_dilate": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "pp_u8_to_frames": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "pp_u8_to_frames_resized": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "pp_resample_coeffs_bicubic": (c_int, [c_int, c_int, c_void_p, c_void_p, c_long]),
     "pp_resample_index_nearest": (c_int, [c_int, c_int, c_void_p]),
     "pp_resample_coeffs_linear_cv": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p]),

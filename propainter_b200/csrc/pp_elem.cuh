@@ -287,10 +287,8 @@ PP_HD float pp_corr_tap_tile(const float* tile, int tx0, int ty0, int Hl, int Wl
 // The rule does exactly that, with explicit roundings; it equals ATen bit for bit on every grid RAFT produces
 // (h, w >= 16; measured with torch 2.11 on x86).  Plain mul-add (no FMA) differs by up to 1 ulp on ~20% of pixels.
 struct PPLin { int i0, i1; float l0, l1; };
-PP_HD PPLin pp_upflow8_coord(int dst, int in) {
-  const int out = 8 * in;
-  const float scale = out > 1 ? PP_DIV((float)(in - 1), (float)(out - 1)) : 0.0f;
-  const float src = PP_MUL(scale, (float)dst);
+// the taps and weights of one source coordinate: i0 = min(floor(src), in-1), l1 = clamp(src - i0, 0, 1)
+PP_HD PPLin pp_lin_taps(float src, int in) {
   PPLin u;
   u.i0 = (int)floorf(src);
   if (u.i0 > in - 1) u.i0 = in - 1;
@@ -299,10 +297,38 @@ PP_HD PPLin pp_upflow8_coord(int dst, int in) {
   u.l0 = PP_SUB(1.0f, u.l1);
   return u;
 }
-PP_HD float pp_upflow8_blend(float v00, float v01, float v10, float v11, const PPLin& uy, const PPLin& ux) {
+PP_HD PPLin pp_upflow8_coord(int dst, int in) {
+  const int out = 8 * in;
+  const float scale = out > 1 ? PP_DIV((float)(in - 1), (float)(out - 1)) : 0.0f;
+  return pp_lin_taps(PP_MUL(scale, (float)dst), in);
+}
+// ATen's separable blend as its x86 build contracts it (see above)
+PP_HD float pp_lin_blend(float v00, float v01, float v10, float v11, const PPLin& uy, const PPLin& ux) {
   const float t0 = PP_FMA(v00, ux.l0, PP_MUL(v01, ux.l1));
   const float t1 = PP_FMA(v10, ux.l0, PP_MUL(v11, ux.l1));
-  return PP_MUL(8.0f, PP_FMA(t0, uy.l0, PP_MUL(t1, uy.l1)));
+  return PP_FMA(t0, uy.l0, PP_MUL(t1, uy.l1));
+}
+PP_HD float pp_upflow8_blend(float v00, float v01, float v10, float v11, const PPLin& uy, const PPLin& ux) {
+  return PP_MUL(8.0f, pp_lin_blend(v00, v01, v10, v11, uy, ux));
+}
+
+// F.interpolate(img, size=(h, w), mode='bilinear', align_corners=False), no antialias (scripts/compute_flow.py:81-89),
+// restated from ATen's CPU upsample_bilinear2d the same way: scale = float(in) / out, src = max(scale * (dst + 0.5) - 0.5,
+// 0) with the x86 build's FMA contraction (fma(scale, dst + 0.5, -0.5)), then the taps and the blend above.  Equals ATen's
+// contiguous NCHW kernel bit for bit on uint8 / 255 frames at every output size RAFT accepts (measured with torch 2.11 on
+// x86: down- and up-scaling, odd source sizes, identity); without the FMA in src about 16% of the values of 720x1280 ->
+// 240x432 differ.  Small outputs (e.g. 74x48) take another ATen code path that differs from this rule by a few ulp.
+// At in == out it picks the source pixel with weight 1 exactly.
+PP_HD PPLin pp_resize_coord(int dst, int in, int out) {
+  const float scale = PP_DIV((float)in, (float)out);
+  return pp_lin_taps(fmaxf(PP_FMA(scale, PP_ADD((float)dst, 0.5f), -0.5f), 0.0f), in);
+}
+// One value of compute_flow.py:67-92 for one channel: ToTensor's v / 255 at each tap, the resize, then img*2 - 1 as two
+// roundings.  At the identity size this is pp_u8_frame.
+PP_HD float pp_u8_frame_resized(uint8_t v00, uint8_t v01, uint8_t v10, uint8_t v11, const PPLin& uy, const PPLin& ux) {
+  const float b = pp_lin_blend(PP_DIV((float)v00, 255.0f), PP_DIV((float)v01, 255.0f), PP_DIV((float)v10, 255.0f),
+                               PP_DIV((float)v11, 255.0f), uy, ux);
+  return PP_SUB(PP_MUL(b, 2.0f), 1.0f);
 }
 
 // RAFT/raft.py:73-84: convex 8x upsampling of one low-res pixel's (i,j) sub-pixel.

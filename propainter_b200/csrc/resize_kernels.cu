@@ -14,10 +14,13 @@
 //   * the evaluation dataset's resize_flow (core/dataset.py:213-214, utils/flow_util.py:6-11): OpenCV's float32
 //     INTER_LINEAR (float coefficients, separable, unfused products and sums; exact 2x down-scaling is its INTER_AREA
 //     fast path) and the per-component rescale, on planar float32 flows [N][2][H][W].
+//   * scripts/compute_flow.py's frame preparation (:67-92): ToTensor, torch F.interpolate(bilinear, align_corners=False)
+//     and *2 - 1, fused into one pass from uint8 frames to RAFT's planar fp32 input (pp_resize_coord in pp_elem.cuh).
 // The uint8 kernels: uint8 [T][H][W][3] (masks [T][H][W]) in, same layout out; stream-ordered; the caller owns tables + scratch.
 #include <math.h>
 #include <stdint.h>
 #include "pp_common.cuh"
+#include "pp_elem.cuh"
 #include "../../include/propainter_b200.h"
 
 #define RS_PREC 22
@@ -283,5 +286,29 @@ extern "C" int pp_resize_flow_linear_cv(const float* src, float* dst, int N, int
     return PP_ERR_SHAPE;
   else
     k_resize_flow_linear<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(src, dst, N, H, W, Ho, Wo, xofs, alpha, yofs, beta, su, sv);
+  return cudaPeekAtLastError() == cudaSuccess ? PP_OK : PP_ERR_LAUNCH;
+}
+
+// scripts/compute_flow.py:67-92 on the device: uint8 RGB [T][H0][W0][3] -> planar fp32 [T][3][h][w] in [-1,1], the rule of
+// pp_resize_coord / pp_u8_frame_resized.  One thread per output pixel, all three channels (the taps of a pixel share rows).
+__global__ void __launch_bounds__(256) k_u8_to_frames_resized(const uint8_t* __restrict__ src, float* __restrict__ dst, int T, int H0,
+                                                              int W0, int h, int w) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long hw = (long)h * w;
+  if (i >= (long)T * hw) return;
+  const int x = (int)(i % w); const long r = i / w; const int y = (int)(r % h); const long t = r / h;
+  const PPLin uy = pp_resize_coord(y, H0, h), ux = pp_resize_coord(x, W0, w);
+  const uint8_t* f = src + t * H0 * W0 * 3;
+  const uint8_t* r0 = f + (long)uy.i0 * W0 * 3;
+  const uint8_t* r1 = f + (long)uy.i1 * W0 * 3;
+  const int x0 = ux.i0 * 3, x1 = ux.i1 * 3;
+  float* o = dst + t * 3 * hw + (long)y * w + x;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) o[c * hw] = pp_u8_frame_resized(r0[x0 + c], r0[x1 + c], r1[x0 + c], r1[x1 + c], uy, ux);
+}
+extern "C" int pp_u8_to_frames_resized(const uint8_t* src, float* dst, int T, int H0, int W0, int h, int w, cudaStream_t stream) {
+  if (T < 1 || H0 < 1 || W0 < 1 || h < 1 || w < 1) return PP_ERR_SHAPE;
+  const long n = (long)T * h * w;
+  k_u8_to_frames_resized<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(src, dst, T, H0, W0, h, w);
   return cudaPeekAtLastError() == cudaSuccess ? PP_OK : PP_ERR_LAUNCH;
 }

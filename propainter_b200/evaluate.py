@@ -154,21 +154,43 @@ def evaluate_flow_clip(pipe, frames_u8, masks_u8, reference_flows=None, cfg=None
         gt = pipe.compute_flows_half(fr.contiguous(), cfg)
     else:
         gt =pipe.compute_flows(ops.u8_to_frames(fr).unsqueeze(0), cfg)
+    return _complete_and_score(pipe, gt, fm, reference_flows, cfg.half_storage)
+
+
+def _complete_and_score(pipe, gt, fm, reference_flows, half):
+    """evaluate_flow_completion.py:111-137 + :141-147: flow completion once over the whole clip, then combine_flow, timed
+    with synchronisations around it; then the EPE of each direction against `reference_flows` (None: against `gt`)."""
+    dev = pipe.device
     net = pipe.fix_flow_complete
     torch.cuda.synchronize(dev)
     t0 = time.perf_counter()
     pred, _ = net.forward_bidirect_flow(gt, fm)
     pred = net.combine_flow(gt, pred, fm)
-    if cfg.half_storage:
+    if half:
         pred = tuple(p.half() for p in pred)
     torch.cuda.synchronize(dev)
     dt = time.perf_counter() - t0
     ref = gt if reference_flows is None else tuple(torch.as_tensor(r).to(dev).float().reshape(p.shape)
                                                    for r, p in zip(reference_flows, pred))
     ef, eb = epe64(ref[0], pred[0]), epe64(ref[1], pred[1])
-    T = fr.shape[0]
+    T = fm.shape[1]
     return {"epe": (ef + eb) / 2, "epe_forward": ef, "epe_backward": eb, "frames": T, "seconds": dt,
             "seconds_per_frame": dt / T, "pred_flows": pred}
+
+
+@torch.no_grad()
+def evaluate_flow_video(pipe, masks, flows):
+    """The per-video body of scripts/evaluate_flow_completion.py:88-160 with --load_flow, on prepare_test_video's outputs:
+    masks float {0,1} [1,T,1,h,w], flows the loaded (forward, backward) pair [T-1,2,h,w] or [1,T-1,2,h,w].  The loaded
+    flows are completed (forward_bidirect_flow + combine_flow over the whole clip) and are also what EPE is measured
+    against.  Returns the record of evaluate_flow_clip: EPE per direction (float64), `seconds` = the synchronised wall
+    time of the completion alone (:111-137), and the completed flows."""
+    dev = pipe.device
+    fm = torch.as_tensor(masks).to(dev).float()
+    T, H, W = fm.shape[1], fm.shape[-2], fm.shape[-1]
+    fm = fm.reshape(1, T, 1, H, W).contiguous()
+    gt = tuple(torch.as_tensor(f).to(dev).float().reshape(1, T - 1, 2, H, W).contiguous() for f in flows)
+    return _complete_and_score(pipe, gt, fm, None, False)
 
 
 def flow_epe_summary(results):
@@ -190,12 +212,13 @@ def prepare_test_video(frames_u8, masks_u8, size, flows=None, device="cuda"):
     args.size.  frames_u8 uint8 [T,H0,W0,3] (RGB) -> [T,h,w,3] by cv2.resize(INTER_LINEAR) -- these frames are both the
     network input and the ground truth; masks_u8 uint8 [T,H0,W0] -> float {0,1} [1,T,1,h,w]: PIL NEAREST resize, > 0,
     cv2.dilate with the 3x3 cross x4; flows: an optional (forward, backward) pair of float32 [T-1,2,Hf,Wf] -> [T-1,2,h,w]
-    through resize_flow (utils/flow_util.py:6-11).  Returns (frames, masks, flows or None).  An exact 2x down-scaling of
+    through resize_flow (utils/flow_util.py:6-11).  Returns (frames, masks, flows or None); frames_u8 = None skips the
+    frames (the flow-completion protocol reads none) and returns None in their place.  An exact 2x down-scaling of
     the frames, where OpenCV switches the 8-bit resize to INTER_AREA, raises (the uint8 kernel does not implement it)."""
     from . import ops
     w, h = (int(s) for s in size)
     dev = torch.device(device)
-    fr = ops.resize_output_u8(torch.as_tensor(frames_u8).to(dev).contiguous(), (w, h))
+    fr = None if frames_u8 is None else ops.resize_output_u8(torch.as_tensor(frames_u8).to(dev).contiguous(), (w, h))
     mk = ops.resize_masks_u8(torch.as_tensor(masks_u8).to(dev).contiguous(), (w, h))
     mk = ops.mask_dilate(mk, 4).unsqueeze(0)
     if flows is not None:
@@ -311,3 +334,72 @@ def evaluate_propainter(pipe, videos, size=(432, 240), task="video_completion", 
     if log:
         log(line)
     return out
+
+
+# ---------------------------------------------------------------- scripts/compute_flow.py and the flow-completion protocol
+@torch.no_grad()
+def compute_flow_video(pipe, frames_u8, size=(432, 240), iters=20):
+    """scripts/compute_flow.py:62-108 for one video after file I/O: the flow ground truth both evaluation scripts load
+    with --load_flow.  frames_u8 uint8 RGB [T,H0,W0,3] (numpy or tensor, T >= 2), size = (w, h), the script's
+    --width / --height (default 432 x 240).  Each frame is resized as the script does (ToTensor, torch bilinear
+    F.interpolate with align_corners=False, *2 - 1: ops.u8_to_frames_resized), then RAFT with `iters` iterations gives
+    the forward flow of every pair (i, i+1) and the backward flow of (i+1, i).
+
+    Returns (forward, backward), each fp16 [T-1,2,h,w] on the pipeline's device: what flowwrite stores, in planar layout
+    (`.float()` of it is flowread's array, transposed to [2,h,w] per pair).  The script runs RAFT once per pair and
+    direction at batch 1; this runs pipe.compute_flows over the whole clip (RAFT's batched chunks and correlation plan),
+    which differs from it only by floating-point summation order.  The result plugs into prepare_test_video(flows=...),
+    evaluate_propainter's and evaluate_flow_completion's videos and evaluate_flow_clip(reference_flows=...)."""
+    from . import ops
+    from .inference_propainter import InferenceConfig
+    w, h = (int(s) for s in size)
+    if w % 8 or h % 8 or w < 128 or h < 128:
+        raise ValueError(f"compute_flow_video: size must be multiples of 8 and at least 128 on both sides (RAFT), got {size}")
+    fr = torch.as_tensor(frames_u8)
+    if fr.dtype != torch.uint8 or fr.dim() != 4 or fr.shape[-1] != 3 or fr.shape[0] < 2:
+        raise ValueError(f"compute_flow_video: expected uint8 frames [T>=2,H,W,3], got {fr.dtype} {tuple(fr.shape)}")
+    frames = ops.u8_to_frames_resized(fr.to(pipe.device).contiguous(), (w, h)).unsqueeze(0)
+    fwd, bwd = pipe.compute_flows(frames, InferenceConfig(raft_iter=iters))
+    return fwd[0].half(), bwd[0].half()
+
+
+def flow_completion_video_line(index, count, name, epe, avg_time):
+    """the per-video line evaluate_flow_completion.py:150-155 prints and writes.  The script prints the name its
+    DataLoader collated (batch_size=1): default_collate transposes the batch with zip, so the name is a one-element
+    tuple and video 'bear' appears as ('bear',).  This prints the same."""
+    return f'[{index + 1:3}/{count}] Name: {str((name,)):25} | EPE: {epe:.4f} | Time: {avg_time:.4f}'
+
+
+def evaluate_flow_completion(pipe, videos, size=(432, 240), log=None):
+    """scripts/evaluate_flow_completion.py::main_worker with --load_flow (:55-179) over `videos`, an iterable of
+    (name, masks_u8, flows) the caller has read: masks uint8 [T,H0,W0], flows the (forward, backward) pair of float32
+    [T-1,2,Hf,Wf] .flo contents (compute_flow_video's output, or flowread's arrays transposed).  Frames are not an input:
+    the script computes nothing from them.  Masks and flows are prepared by prepare_test_video at size = (w, h) and each
+    video is scored by evaluate_flow_video.  flows = None raises ValueError: the script cannot run without --load_flow.
+
+    Returns {"videos": per-video records (name, EPE per direction and their mean `epe`, seconds, the running mean time
+    per frame avg_time, line = the script's text), "summary": flow_epe_summary of the records, "line": the script's
+    final line}.  `log(text)` receives each line as it is produced.  The completed flows are not kept."""
+    recs = []
+    videos = list(videos)
+    for name, _, flows in videos:
+        if flows is None:
+            raise ValueError(f"evaluate_flow_completion: video {name!r} has no flows (the protocol runs on loaded flows)")
+    frames = seconds = 0
+    for index, (name, masks_u8, flows) in enumerate(videos):
+        torch.cuda.empty_cache()
+        _, mk, fl = prepare_test_video(None, masks_u8, size, flows, pipe.device)
+        r = evaluate_flow_video(pipe, mk, fl)
+        r.pop("pred_flows")
+        frames += r["frames"]
+        seconds += r["seconds"]
+        r.update(name=name, avg_time=seconds / frames)
+        r["line"] = flow_completion_video_line(index, len(videos), name, r["epe"], r["avg_time"])
+        if log:
+            log(r["line"])
+        recs.append(r)
+    s = flow_epe_summary(recs)
+    line = f'Finish evaluation... Average Frame EPE: {s["epe"]:.4f} | | Time: {s["seconds_per_frame"]:.4f}'
+    if log:
+        log(line)
+    return {"videos": recs, "summary": s, "line": line}

@@ -719,6 +719,23 @@ def u8_to_frames(frames_u8):
     return out
 
 
+def u8_to_frames_resized(frames_u8, size):
+    """scripts/compute_flow.py:67-92: uint8 RGB [T,H0,W0,3] -> float planar [T,3,h,w] in [-1,1], size = (w, h): v / 255,
+    torch's bilinear F.interpolate (align_corners=False, no antialias), then *2 - 1.  Bit for bit with that sequence on
+    ATen's CPU kernel; at the frames' own size equal to u8_to_frames."""
+    if frames_u8.dtype != torch.uint8 or frames_u8.dim() != 4 or frames_u8.shape[-1] != 3 or frames_u8.shape[0] < 1:
+        raise ValueError(f"u8_to_frames_resized: expected uint8 frames [T,H,W,3], got {frames_u8.dtype} {tuple(frames_u8.shape)}")
+    w, h = (int(s) for s in size)
+    T, H0, W0, _ = frames_u8.shape
+    if w < 1 or h < 1 or H0 < 1 or W0 < 1:
+        raise ValueError(f"u8_to_frames_resized: cannot resize {H0}x{W0} frames to size {tuple(size)}")
+    out = torch.empty(T, 3, h, w, device=frames_u8.device, dtype=torch.float32)
+    check(_lib.lib().pp_u8_to_frames_resized(_p(_dense(frames_u8), torch.uint8), _p(out), T, H0, W0, h, w, _stream()),
+          "pp_u8_to_frames_resized")
+    _count(1)
+    return out
+
+
 def composite_blend(pred, masks, ori_u8, comp_u8, frame_ids, first_flags):
     """pred [n,3,H,W]; masks [T,1,H,W]; ori/comp uint8 [T,H,W,3] (comp updated in place)."""
     n, _, H, W = pred.shape
