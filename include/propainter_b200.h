@@ -372,6 +372,24 @@ int pp_flow_maxrad(const float* flow, float* maxima, int N, int H, int W, int pe
  * pp_flow_maxrad with the matching per_frame -> uint8 out [N][H][W][3], RGB (BGR when bgr). */
 int pp_flow_to_image_u8(const float* flow, const float* maxima, uint8_t* out, int N, int H, int W, int variant, int has_clip,
                         float clip_flow, int bgr, cudaStream_t stream);
+/* ---- temporal warping error E_warp ------------------------------------------------------------------------------- */
+/* No reference line: the reference defers this metric to the evaluation of Lai et al., "Learning Blind Video Temporal
+ * Consistency" (ECCV 2018), whose occlusion test is that of Ruder et al., "Artistic style transfer for videos" (GCPR
+ * 2016).  Warps are FlowNet2 Resample2d's border-clamped bilinear sample (pp_clamp_taps in pp_elem.cuh).
+ * Flows planar float32 [N][2][H][W], pair t: fw frame t -> t+1, bw frame t+1 -> t.
+ * Occlusion map O_t -> occ uint8 [N][H][W], 1 = occluded: |F + w|^2 > 0.01 (|F|^2 + |w|^2) + 0.5 with w = bw sampled at
+ * x + F(x), or the motion-boundary test |du|^2 + |dv|^2 > 0.01 |F|^2 + 0.002 (forward differences, 0 in the last
+ * column / row).  PP_ERR_SHAPE unless N, H, W >= 1. */
+int pp_flow_occlusion(const float* fw, const float* bw, uint8_t* occ, int N, int H, int W, cudaStream_t stream);
+/* Per pair t of frames uint8 [T][H][W][3] (values / 255): out float64 [T-1][2] = (sum over pixels with O_t = 0 of
+ * sum_c (S(frame t+1, fw_t) - frame t)^2, N_t = their count); E_t = sum / (3 N_t).  O_t is read from occ (uint8
+ * [T-1][H][W], non-zero = occluded; bw unused, may be NULL) or, when occ is NULL, computed from fw / bw in the same pass.
+ * fp32 per pixel, float64 sums in a fixed order without atomics: the same bits on every run.  Caller-owned workspace of
+ * pp_warp_error_workspace_bytes(T, H, W) bytes (0 for an invalid shape).  PP_ERR_SHAPE unless 2 <= T <= 65536, H, W >= 1
+ * and occ or bw is given. */
+size_t pp_warp_error_workspace_bytes(int T, int H, int W);
+int pp_warp_error(const uint8_t* frames, const float* fw, const float* bw, const uint8_t* occ, double* out, int T, int H, int W,
+                  void* workspace, size_t workspace_bytes, cudaStream_t stream);
 /* ---- I3D feature network of VFID (core/metrics.py:62-82,195-569) ---------------------------------------------- */
 /* 'same' padding (Unit3D / MaxPool3dSamePadding.compute_pad, core/metrics.py:196-200,258-262): for a k-tap window of stride
  * s over n samples, pad = max(k - (n % s ? n % s : s), 0), front pad / 2, back the rest (pp_same_pad in pp_elem.cuh);

@@ -145,6 +145,9 @@ SIGNATURES = {
     "pp_mask_overlay_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "pp_flow_maxrad": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [ctypes.c_float, c_void_p]),
     "pp_flow_to_image_u8": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [ctypes.c_float, c_int, c_void_p]),
+    "pp_flow_occlusion": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "pp_warp_error_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "pp_warp_error": (c_int, [c_void_p] * 5 + [c_int] * 3 + [c_void_p, c_size_t, c_void_p]),
     "pp_i3d_input": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "pp_maxpool3d_same": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_int] * 11 + [c_void_p]),
     "pp_mean_thw": (c_int, [c_void_p, c_int, c_void_p, c_int, c_long, c_int, c_void_p]),

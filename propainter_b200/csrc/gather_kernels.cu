@@ -1317,3 +1317,105 @@ extern "C" int pp_flow_to_image_u8(const float* flow, const float* maxima, uint8
   PP_LAUNCH_CHECK();
   return PP_OK;
 }
+
+// ================================================================ temporal warping error (E_warp)
+// Lai et al. (ECCV 2018) with the occlusion test of Ruder et al. (GCPR 2016); the per-pixel rules are pp_clamp_taps /
+// pp_flow_occluded / pp_warp_sqdiff of pp_elem.cuh.  Flows planar float32 [T-1][2][H][W], frames uint8 [T][H][W][3].
+// grid (pixel blocks, N); per-frame offsets in 32 bits (a frame's H * W * 3 < 2^31), the pair's base in 64
+__global__ void __launch_bounds__(256) k_flow_occlusion(const float* __restrict__ fw, const float* __restrict__ bw,
+                                                        uint8_t* __restrict__ occ, int H, int W) {
+  const int HW = H * W, p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= HW) return;
+  const long n = blockIdx.y;
+  const int y = p / W, x = p - y * W;
+  const float* F = fw + n * 2 * HW;
+  const PPClampTaps t = pp_clamp_taps(x, y, F[p], F[HW + p], H, W);
+  occ[n * HW + p] = (uint8_t)pp_flow_occluded(F, bw + n * 2 * HW, t, x, y, H, W);
+}
+// O_t of every pair -> occ uint8 [N][H][W], 1 = occluded
+extern "C" int pp_flow_occlusion(const float* fw, const float* bw, uint8_t* occ, int N, int H, int W, cudaStream_t stream) {
+  if (N < 1 || N > 65535 || H < 1 || W < 1 || (long)H * W * 3 > 0x7fffffffL) return PP_ERR_SHAPE;
+  k_flow_occlusion<<<dim3(pp_blocks((long)H * W, 256), N), 256, 0, stream>>>(fw, bw, occ, H, W);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+
+// Blocks per pair of k_warp_error: a function of the frame size alone, so the grid, each thread's pixels and the
+// summation order are the same on every run and every device (no atomics: the sums are bit-reproducible).
+static inline int pp_ewarp_blocks(long HW) { const int b = pp_blocks(HW, 256); return b < 1024 ? b : 1024; }
+
+// a fixed-order sum of one double per thread of a 256-thread block; the total lands in thread 0
+__device__ __forceinline__ double pp_block_sum_f64(double v, double* red) {
+  for (int o = 16; o > 0; o >>= 1) v = PP_DADD(v, __shfl_down_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (int k = 1; k < 8; ++k) v = PP_DADD(v, red[k]);
+  __syncthreads();
+  return v;
+}
+
+// grid (blocks, T-1): each block strides over the pixels of pair t, keeps the non-occluded ones (from `occ`, or the
+// test computed from `bw` when occ is NULL), and writes (sum of squared differences, count) in float64 to part
+__global__ void __launch_bounds__(256) k_warp_error(const uint8_t* __restrict__ frames, const float* __restrict__ fw,
+                                                    const float* __restrict__ bw, const uint8_t* __restrict__ occ,
+                                                    double* __restrict__ part, int H, int W) {
+  __shared__ double red[8];
+  const long pair = blockIdx.y;
+  const int HW = H * W;
+  const float* F = fw + pair * 2 * HW;
+  const uint8_t* cur = frames + pair * HW * 3;
+  const uint8_t* next = cur + HW * 3;
+  double s = 0.0, n = 0.0;
+  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += gridDim.x * blockDim.x) {
+    const int y = p / W, x = p - y * W;
+    const PPClampTaps t = pp_clamp_taps(x, y, F[p], F[HW + p], H, W);
+    const int o = occ ? occ[pair * HW + p] != 0 : pp_flow_occluded(F, bw + pair * 2 * HW, t, x, y, H, W);
+    if (!o) {
+      s = PP_DADD(s, (double)pp_warp_sqdiff(next, cur, t, p));
+      n = PP_DADD(n, 1.0);
+    }
+  }
+  s = pp_block_sum_f64(s, red);
+  n = pp_block_sum_f64(n, red);
+  if (threadIdx.x == 0) {
+    double* o = part + ((long)pair * gridDim.x + blockIdx.x) * 2;
+    o[0] = s;
+    o[1] = n;
+  }
+}
+// one block per pair: the block partials in a fixed order -> out [T-1][2]
+__global__ void __launch_bounds__(256) k_warp_error_reduce(const double* __restrict__ part, double* __restrict__ out, int nblk) {
+  __shared__ double red[8];
+  const double* p = part + (long)blockIdx.x * nblk * 2;
+  double s = 0.0, n = 0.0;
+  for (int b = threadIdx.x; b < nblk; b += blockDim.x) {
+    s = PP_DADD(s, p[2 * b]);
+    n = PP_DADD(n, p[2 * b + 1]);
+  }
+  s = pp_block_sum_f64(s, red);
+  n = pp_block_sum_f64(n, red);
+  if (threadIdx.x == 0) {
+    out[2 * blockIdx.x] = s;
+    out[2 * blockIdx.x + 1] = n;
+  }
+}
+
+extern "C" size_t pp_warp_error_workspace_bytes(int T, int H, int W) {
+  if (T < 2 || H < 1 || W < 1) return 0;
+  return (size_t)(T - 1) * pp_ewarp_blocks((long)H * W) * 2 * sizeof(double);
+}
+// (sum, N_t) of the warping error of every pair (t, t+1) -> out float64 [T-1][2]
+extern "C" int pp_warp_error(const uint8_t* frames, const float* fw, const float* bw, const uint8_t* occ, double* out, int T, int H,
+                             int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (T < 2 || T - 1 > 65535 || H < 1 || W < 1 || (long)H * W * 3 > 0x7fffffffL) return PP_ERR_SHAPE;
+  if (!occ && !bw) return PP_ERR_SHAPE;
+  if (workspace_bytes < pp_warp_error_workspace_bytes(T, H, W)) return PP_ERR_WORKSPACE;
+  const int nblk = pp_ewarp_blocks((long)H * W);
+  double* part = (double*)workspace;
+  k_warp_error<<<dim3(nblk, T - 1), 256, 0, stream>>>(frames, fw, occ ? nullptr : bw, occ, part, H, W);
+  PP_LAUNCH_CHECK();
+  k_warp_error_reduce<<<T - 1, 256, 0, stream>>>(part, out, nblk);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}

@@ -591,3 +591,72 @@ PP_HD int pp_same_out(int k, int s, int n) { return (n + pp_same_pad(k, s, n) - 
 // one tap of ATen's max pooling (max_pool3d_with_indices): a larger value or a NaN replaces the running maximum, so
 // the first NaN sticks and, among equal values (+0 / -0), the first tap in (t, y, x) order wins
 PP_HD float pp_pool_max(float m, float v) { return (v > m || isnan(v)) ? v : m; }
+
+// ---- temporal warping error (Lai et al., "Learning Blind Video Temporal Consistency", ECCV 2018) ----
+// Border-clamped bilinear sample of FlowNet2's Resample2d, the warp of Lai et al.'s evaluation: pixel (x, y) moved by
+// (fx, fy) in float32; taps floor and floor + 1 on each axis, each clamped into the frame; weights from the unclamped
+// fractions a, b.  Far outside the frame this returns the border pixel (not grid_sample's zeros of pp_taps).  Indices
+// are clamped in float, so a huge or NaN coordinate cannot overflow the int conversion.  32-bit pixel indices: one
+// frame's H * W * 3 stays below 2^31.
+struct PPClampTaps {
+  int i00, i01, i10, i11;         // pixel indices y * W + x of (yT, xL) (yT, xR) (yB, xL) (yB, xR)
+  float w00, w01, w10, w11;       // (1-a)(1-b), a(1-b), (1-a)b, ab
+};
+PP_HD PPClampTaps pp_clamp_taps(int x, int y, float fx, float fy, int H, int W) {
+  const float xf = PP_ADD((float)x, fx), yf = PP_ADD((float)y, fy);
+  const float flx = floorf(xf), fly = floorf(yf);
+  const float a = PP_SUB(xf, flx), b = PP_SUB(yf, fly);
+  const float wm = (float)(W - 1), hm = (float)(H - 1);
+  const int xl = (int)fminf(fmaxf(flx, 0.0f), wm), xr = (int)fminf(fmaxf(PP_ADD(flx, 1.0f), 0.0f), wm);
+  const int yt = (int)fminf(fmaxf(fly, 0.0f), hm), yb = (int)fminf(fmaxf(PP_ADD(fly, 1.0f), 0.0f), hm);
+  PPClampTaps t;
+  t.i00 = yt * W + xl; t.i01 = yt * W + xr; t.i10 = yb * W + xl; t.i11 = yb * W + xr;
+  const float ra = PP_SUB(1.0f, a), rb = PP_SUB(1.0f, b);
+  t.w00 = PP_MUL(ra, rb); t.w01 = PP_MUL(a, rb); t.w10 = PP_MUL(ra, b); t.w11 = PP_MUL(a, b);
+  return t;
+}
+// a value as the warp reads it: flow components as they are, uint8 frame values as v / 255 in float32
+PP_HD float pp_ewarp_load(float v) { return v; }
+PP_HD float pp_ewarp_load(uint8_t v) { return PP_DIV((float)v, 255.0f); }
+// one channel of a plane whose pixels are `stride` elements apart, sampled through a tap set in Resample2d's order
+template <typename T>
+PP_HD float pp_clamp_sample(const T* p, int stride, const PPClampTaps& t) {
+  float acc = PP_MUL(t.w00, pp_ewarp_load(p[t.i00 * stride]));
+  acc = PP_ADD(acc, PP_MUL(t.w01, pp_ewarp_load(p[t.i01 * stride])));
+  acc = PP_ADD(acc, PP_MUL(t.w10, pp_ewarp_load(p[t.i10 * stride])));
+  return PP_ADD(acc, PP_MUL(t.w11, pp_ewarp_load(p[t.i11 * stride])));
+}
+// occlusion test 1 of Ruder et al. ("Artistic style transfer for videos", GCPR 2016), forward-backward consistency:
+// occluded where |F + w|^2 > 0.01 (|F|^2 + |w|^2) + 0.5, w = B sampled at x + F(x); squared magnitudes, no root
+PP_HD int pp_occ_fb(float fx, float fy, float wx, float wy) {
+  const float sx = PP_ADD(fx, wx), sy = PP_ADD(fy, wy);
+  const float lhs = PP_ADD(PP_MUL(sx, sx), PP_MUL(sy, sy));
+  const float mag = PP_ADD(PP_ADD(PP_MUL(fx, fx), PP_MUL(fy, fy)), PP_ADD(PP_MUL(wx, wx), PP_MUL(wy, wy)));
+  return lhs > PP_ADD(PP_MUL(0.01f, mag), 0.5f);
+}
+// occlusion test 2 (motion boundary): du = F(y, x) - F(y, x+1), dv = F(y, x) - F(y+1, x) per component (0 in the last
+// column / row); occluded where du_x^2 + dv_x^2 + du_y^2 + dv_y^2 > 0.01 |F|^2 + 0.002
+PP_HD int pp_occ_motion(float dux, float dvx, float duy, float dvy, float fx, float fy) {
+  const float lhs = PP_ADD(PP_ADD(PP_ADD(PP_MUL(dux, dux), PP_MUL(dvx, dvx)), PP_MUL(duy, duy)), PP_MUL(dvy, dvy));
+  return lhs > PP_ADD(PP_MUL(0.01f, PP_ADD(PP_MUL(fx, fx), PP_MUL(fy, fy))), 0.002f);
+}
+// the occlusion map O_t at pixel p = (x, y) of one pair: F, B planar [2][H][W] (forward t -> t+1, backward t+1 -> t),
+// `t` the tap set of x + F(x).  1 = occluded (either test).
+PP_HD int pp_flow_occluded(const float* F, const float* B, const PPClampTaps& t, int x, int y, int H, int W) {
+  const int HW = H * W, p = y * W + x;
+  const float fx = F[p], fy = F[HW + p];
+  if (pp_occ_fb(fx, fy, pp_clamp_sample(B, 1, t), pp_clamp_sample(B + HW, 1, t))) return 1;
+  const float dux = x + 1 < W ? PP_SUB(fx, F[p + 1]) : 0.0f, duy = x + 1 < W ? PP_SUB(fy, F[HW + p + 1]) : 0.0f;
+  const float dvx = y + 1 < H ? PP_SUB(fx, F[p + W]) : 0.0f, dvy = y + 1 < H ? PP_SUB(fy, F[HW + p + W]) : 0.0f;
+  return pp_occ_motion(dux, dvx, duy, dvy, fx, fy);
+}
+// per-pixel squared difference of the warping error: sum over RGB of (S(next / 255, F)(p) - cur(p) / 255)^2, frames
+// uint8 pixel-major [H][W][3]
+PP_HD float pp_warp_sqdiff(const uint8_t* next, const uint8_t* cur, const PPClampTaps& t, int p) {
+  float s = 0.0f;
+  for (int c = 0; c < 3; ++c) {
+    const float d = PP_SUB(pp_clamp_sample(next + c, 3, t), pp_ewarp_load(cur[p * 3 + c]));
+    s = PP_ADD(s, PP_MUL(d, d));
+  }
+  return s;
+}

@@ -227,8 +227,36 @@ def prepare_test_video(frames_u8, masks_u8, size, flows=None, device="cuda"):
 
 
 @torch.no_grad()
+def warp_error(result_u8, flows):
+    """The temporal warping error E_warp of Lai et al., "Learning Blind Video Temporal Consistency" (ECCV 2018), which the
+    reference's README defers to for --save_results output, with the occlusion test of Ruder et al. (GCPR 2016).
+    result_u8 uint8 [T,H,W,3] (the saved frames; values / 255), flows the (forward, backward) pair of the ground-truth
+    clip, each [T-1,2,H,W] or [1,T-1,2,H,W] in fp32 or fp16 (RAFT's, or compute_flow_video's).  Per pair t, frame t+1
+    is warped to frame t along the forward flow (border-clamped bilinear), and E_t is the mean squared RGB difference
+    over the pixels the occlusion test keeps (0 if it keeps none).  One device pass (ops.warp_error_sums).
+
+    Returns {"ewarp": mean over pairs of E_t, "ewarp_per_pair": [E_t], "occluded_fraction": share of occluded pixels
+    over all pairs}, raw values (no x 1e-3).  Comparable across methods scored by this package; not digit for digit
+    with published tables, which used FlowNet2 flows on frames resized to multiples of 64 (INTEGRATION.md §3)."""
+    from . import ops
+    fw, bw = flows
+    dev = result_u8.device if isinstance(result_u8, torch.Tensor) else torch.device("cuda")
+    fr = torch.as_tensor(result_u8).to(dev)
+    fw, bw = (torch.as_tensor(f).to(dev) for f in (fw, bw))
+    sums = ops.warp_error_sums(fr, fw, bw=bw).cpu()
+    s, n = sums[:, 0].tolist(), sums[:, 1].tolist()
+    per_pair = [a / (3 * k) if k > 0 else 0.0 for a, k in zip(s, n)]
+    T, H, W = fr.shape[0], fr.shape[1], fr.shape[2]
+    return {"ewarp": sum(per_pair) / len(per_pair), "ewarp_per_pair": per_pair,
+            "occluded_fraction": 1.0 - sum(n) / ((T - 1) * H * W)}
+
+
+_warp_error = warp_error            # evaluate_video's argument of the same name shadows it there
+
+
+@torch.no_grad()
 def evaluate_video(pipe, frames_u8, masks, flows=None, task="video_completion", neighbor_length=20, ref_stride=10,
-                   raft_iter=20, i3d=None, cfg=None):
+                   raft_iter=20, i3d=None, cfg=None, warp_error=False):
     """The per-video body of scripts/evaluate_propainter.py::main_worker (:92-210) on prepare_test_video's outputs:
     frames_u8 uint8 [T,h,w,3], masks float {0,1} [1,T,1,h,w] (one mask set for flow completion, propagation, the
     generator and compositing), flows the loaded (forward, backward) pair [T-1,2,h,w] or [1,T-1,2,h,w] (--load_flow),
@@ -241,7 +269,10 @@ def evaluate_video(pipe, frames_u8, masks, flows=None, task="video_completion", 
     compositing (:100-101, :181-184).  video_completion: per-frame PSNR / SSIM in float64 of the float frames against
     the input frames, and with `i3d` (an InceptionI3d) the pair (real, comp truncated to uint8) of I3D activations.
     object_removal only times.  `cfg`: an InferenceConfig for what the script leaves open (windows_in_flight); its
-    schedule fields are replaced by the protocol's, and half_storage raises ValueError (the script has no such mode)."""
+    schedule fields are replaced by the protocol's, and half_storage raises ValueError (the script has no such mode).
+    `warp_error`: also the temporal warping error of the result (the module's warp_error, keys ewarp / ewarp_per_pair /
+    occluded_fraction) on comp truncated to uint8, with the protocol's ground-truth flows (RAFT's or the loaded ones),
+    which are then kept until after the timed region; either task."""
     from dataclasses import replace
     from . import ops
     from .inference_propainter import InferenceConfig
@@ -264,7 +295,7 @@ def evaluate_video(pipe, frames_u8, masks, flows=None, task="video_completion", 
     else:
         gt = pipe.compute_flows(frames, cfg)
     pred = pipe.complete_flows(gt, mk, cfg)                       # subvideo_length >= T: one pass over the clip
-    del gt
+    gt = (gt[0][0], gt[1][0]) if warp_error else None
     prop, upd_m = pipe.model.img_propagation(frames * (1 - mk), pred, mk, "nearest")
     upd_f = frames * (1 - mk) + prop * mk
     del prop, frames
@@ -278,6 +309,8 @@ def evaluate_video(pipe, frames_u8, masks, flows=None, task="video_completion", 
         out.update(psnr_per_frame=ps, ssim_per_frame=ss, psnr=sum(ps) / len(ps), ssim=sum(ss) / len(ss))
         if i3d is not None:
             out["i3d"] = (i3d_activations(i3d, ori), i3d_activations(i3d, comp.to(torch.uint8)))
+    if warp_error:
+        out.update(_warp_error(comp.to(torch.uint8), gt))
     return out
 
 
@@ -291,7 +324,7 @@ def protocol_video_line(index, count, name, rec, avg_psnr, avg_ssim, avg_time):
 
 
 def evaluate_propainter(pipe, videos, size=(432, 240), task="video_completion", neighbor_length=20, ref_stride=10,
-                        raft_iter=20, i3d=None, cfg=None, log=None):
+                        raft_iter=20, i3d=None, cfg=None, log=None, warp_error=False):
     """scripts/evaluate_propainter.py::main_worker's dataset loop over `videos`, an iterable of (name, frames_u8,
     masks_u8, flows) the caller has read (frames uint8 [T,H0,W0,3] RGB, masks uint8 [T,H0,W0], flows None or the
     (forward, backward) pair of float32 [T-1,2,Hf,Wf] .flo contents), each prepared by prepare_test_video at
@@ -301,14 +334,16 @@ def evaluate_propainter(pipe, videos, size=(432, 240), task="video_completion", 
     avg_ssim, the running mean time per frame avg_time, per-frame metrics, seconds, line = the script's text),
     "summary": video_completion_summary of the records (PSNR / SSIM over all frames, VFID with `i3d`, mean time per
     frame), "line": the script's final line}.  `log(text)` receives each line as it is produced.  The composited
-    videos are not kept."""
+    videos are not kept.  `warp_error`: each record also holds evaluate_video's warping-error keys, summary["ewarp"] is
+    their mean over videos (not frame-weighted), and out["ewarp_line"] = "Average Warping Error = ..." follows the final
+    line; the script's lines are unchanged."""
     recs = []
     videos = list(videos)
     frame_psnr, frame_ssim, times = [], [], []
     for index, (name, frames_u8, masks_u8, flows) in enumerate(videos):
         torch.cuda.empty_cache()
         fr, mk, fl = prepare_test_video(frames_u8, masks_u8, size, flows, pipe.device)
-        r = evaluate_video(pipe, fr, mk, fl, task, neighbor_length, ref_stride, raft_iter, i3d, cfg)
+        r = evaluate_video(pipe, fr, mk, fl, task, neighbor_length, ref_stride, raft_iter, i3d, cfg, warp_error)
         r.pop("comp")
         times.append(r["seconds_per_frame"])
         avg_time = sum(times) / len(times)
@@ -333,6 +368,11 @@ def evaluate_propainter(pipe, videos, size=(432, 240), task="video_completion", 
     out.update(summary=s, line=line)
     if log:
         log(line)
+    if warp_error:
+        s["ewarp"] = sum(r["ewarp"] for r in recs) / len(recs)
+        out["ewarp_line"] = f'Average Warping Error = {s["ewarp"]:.6f}'
+        if log:
+            log(out["ewarp_line"])
     return out
 
 

@@ -831,6 +831,83 @@ def flow_to_image_u8(flow, normalize="frame", clip_flow=None, bgr=False):
     return out[0] if single else out
 
 
+# ---------------------------------------------------------------- temporal warping error (E_warp)
+def _ewarp_flows(flow, what):
+    """[N,2,H,W] or [1,N,2,H,W], fp32 or fp16 -> [N,2,H,W] (shape and dtype checked; the device is checked by _ewarp_dev)"""
+    if not isinstance(flow, torch.Tensor):
+        raise ValueError(f"{what}: flows must be a torch tensor, got {type(flow).__name__}")
+    f = flow[0] if flow.dim() == 5 and flow.shape[0] == 1 else flow
+    if f.dim() != 4 or f.shape[1] != 2 or f.dtype not in (torch.float32, torch.float16):
+        raise ValueError(f"{what}: expected fp32 / fp16 flows [N,2,H,W] or [1,N,2,H,W], got {flow.dtype} {tuple(flow.shape)}")
+    if f.shape[0] < 1 or f.shape[2] < 1 or f.shape[3] < 1:
+        raise ValueError(f"{what}: empty flows {tuple(flow.shape)}")
+    return f
+
+
+def _ewarp_dev(what, *tensors):
+    """raise ValueError unless every tensor is on the device; fp16 flows are widened here, once"""
+    if not all(t.is_cuda for t in tensors if t is not None):
+        raise ValueError(f"{what}: inputs must be CUDA tensors (there is no CPU path)")
+    return [None if t is None else t.float().contiguous() if t.is_floating_point() else t.contiguous() for t in tensors]
+
+
+def flow_occlusion(fw, bw):
+    """Occlusion maps of Lai et al.'s warping-error evaluation (the test of Ruder et al.): forward flows fw (frame t ->
+    t+1) and backward flows bw (t+1 -> t), each [N,2,H,W] or [1,N,2,H,W] in fp32 or fp16 -> uint8 [N,H,W], 1 = occluded
+    (forward-backward check or motion boundary; include/propainter_b200.h)."""
+    f, b = _ewarp_flows(fw, "flow_occlusion"), _ewarp_flows(bw, "flow_occlusion")
+    if f.shape != b.shape:
+        raise ValueError(f"flow_occlusion: forward {tuple(fw.shape)} and backward {tuple(bw.shape)} flows differ in shape")
+    f, b = _ewarp_dev("flow_occlusion", f, b)
+    N, _, H, W = f.shape
+    occ = torch.empty(N, H, W, dtype=torch.uint8, device=f.device)
+    check(_lib.lib().pp_flow_occlusion(_p(f), _p(b), _p(occ, torch.uint8), N, H, W, _stream()), "pp_flow_occlusion")
+    _count(1)
+    return occ
+
+
+def warp_error_sums(frames_u8, fw, occ=None, bw=None):
+    """The kernel's per-pair result: float64 [T-1,2] = (sum over the non-occluded pixels and RGB of the squared
+    difference between frame t+1 warped by fw_t and frame t, both / 255; N_t = the number of those pixels).  frames uint8
+    [T,H,W,3] on the device, T >= 2; fw as for flow_occlusion with N = T-1.  The occlusion map is `occ` (uint8
+    [T-1,H,W], non-zero = occluded) or, without it, computed from `bw` in the same pass.  Fixed-order float64 sums: the
+    same bits on every run."""
+    if not isinstance(frames_u8, torch.Tensor) or frames_u8.dtype != torch.uint8 or frames_u8.dim() != 4 or frames_u8.shape[-1] != 3:
+        raise ValueError(f"warp_error: expected uint8 frames [T,H,W,3], got {getattr(frames_u8, 'dtype', type(frames_u8))} "
+                         f"{tuple(getattr(frames_u8, 'shape', ()))}")
+    T, H, W, _ = frames_u8.shape
+    if T < 2 or H < 1 or W < 1:
+        raise ValueError(f"warp_error: needs at least 2 non-empty frames, got {tuple(frames_u8.shape)}")
+    f = _ewarp_flows(fw, "warp_error")
+    if tuple(f.shape) != (T - 1, 2, H, W):
+        raise ValueError(f"warp_error: flows {tuple(fw.shape)} do not match frames {tuple(frames_u8.shape)}")
+    b = None
+    if occ is not None:
+        if not isinstance(occ, torch.Tensor) or occ.dtype != torch.uint8 or tuple(occ.shape) != (T - 1, H, W):
+            raise ValueError(f"warp_error: occ must be a uint8 tensor [{T - 1},{H},{W}]")
+    elif bw is not None:
+        b = _ewarp_flows(bw, "warp_error")
+        if b.shape != f.shape:
+            raise ValueError(f"warp_error: backward flows {tuple(bw.shape)} do not match forward flows {tuple(fw.shape)}")
+    else:
+        raise ValueError("warp_error: needs the occlusion map `occ` or the backward flows `bw`")
+    fr, f, b, o = _ewarp_dev("warp_error", frames_u8, f, b, occ)
+    L = _lib.lib()
+    ws = torch.empty(L.pp_warp_error_workspace_bytes(T, H, W), dtype=torch.uint8, device=f.device)
+    out = torch.empty(T - 1, 2, dtype=torch.float64, device=f.device)
+    check(L.pp_warp_error(_p(fr, torch.uint8), _p(f), _p(b), _p(o, torch.uint8), _p(out, torch.float64), T, H, W,
+                          _p(ws, torch.uint8), ws.numel(), _stream()), "pp_warp_error")
+    _count(2)
+    return out
+
+
+def warp_error(frames_u8, fw, occ=None, bw=None):
+    """Per-pair temporal warping error E_t of Lai et al. (ECCV 2018), float64 [T-1] on the device: warp_error_sums'
+    sum / (3 N_t), 0 where every pixel is occluded.  Frames [0, 1] scale (no x 1e-3)."""
+    s = warp_error_sums(frames_u8, fw, occ, bw)
+    return torch.where(s[:, 1] > 0, s[:, 0] / (3 * s[:, 1]).clamp(min=1), torch.zeros_like(s[:, 0]))
+
+
 # ---------------------------------------------------------------- I3D feature network (VFID)
 def same_pad(k, s, n):
     """TF 'same' padding of a k-tap, stride-s window over n samples (pp_same_pad, core/metrics.py:196-200,258-262); the front
