@@ -408,6 +408,28 @@ int pp_maxpool3d_same(const float* x, int ld_x, float* out, int ld_out, int B, i
  * (N = T*H*W pixels) -> out float [B][C], summed in float64 in a fixed order and rounded once. */
 int pp_mean_thw(const float* x, int ld, float* out, int B, long N, int C, cudaStream_t stream);
 
+/* ---- Cutie mask tracker (web-demos/hugging_face/tracker) ------------------------------------------------------------ */
+/* The working-memory read of MemoryManager.read / _readout (tracker/inference/memory_manager.py:160-187,68-79) at top_k:
+ * get_similarity (anisotropic L2, tracker/model/utils/memory_utils.py:6-42) of every memory token against each query
+ * column, do_softmax's top-k + softmax (:45-73) and the bmm with each object's values, in one pass: neither the N x HW
+ * similarity nor the dense affinity exists.  Memory lives in ring buffers of 1 + fifo_cap frame slots of HW tokens:
+ * mem_key [slots*HW][64], mem_shrink [slots*HW], mem_value [num_objects][slots*HW][256] (object o at
+ * o * value_obj_stride floats); slot 0 is the permanent frame, logical frame f >= 1 is slot 1 + (fifo_head + f - 1) %
+ * fifo_cap, and n_frames frames are read (N = n_frames * HW tokens, in the reference's order).  qk, qe planar [64][HW];
+ * out pixel-major [num_objects][HW][256]; mem_key, mem_value, out 16-byte aligned.  top_k <= 32; when N < top_k all N
+ * tokens are kept.  Ties keep the lower token index (csrc/pp_topk.cuh).  sel_idx / sel_w (both or neither,
+ * [HW][top_k]): the selected logical tokens in descending order and their softmax weights, -1 / 0 past min(top_k, N).  fp32 CUDA-core arithmetic throughout. */
+int pp_cutie_topk_readout(const float* mem_key, const float* mem_shrink, const float* mem_value, long value_obj_stride,
+                          int n_frames, int fifo_head, int fifo_cap, const float* qk, const float* qe, int HW, int num_objects,
+                          int top_k, float* out, int* sel_idx, float* sel_w, cudaStream_t stream);
+/* image_to_torch + pad_divide_by(16) + encode_image's normalisation (base_tracker.py:46-51, tracker/utils/tensor_utils.py:6-21,
+ * tracker/model/cutie.py:59-62): uint8 frame [H][W][3] -> float planar [3][Hp][Wp], Hp / Wp the next multiples of 16,
+ * the zero padding (floor half before) normalised as the reference's is. */
+int pp_cutie_frame_in(const uint8_t* frame, float* out, int H, int W, cudaStream_t stream);
+/* torch.argmax over K probability channels [K][Hp][Wp] (padded as pp_cutie_frame_in), unpad and the MaskMapper remapping
+ * lut[K] (base_tracker.py:79-87) -> uint8 labels [H][W]. */
+int pp_cutie_labels(const float* prob, int K, const uint8_t* lut, uint8_t* out, int H, int W, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -151,6 +151,10 @@ SIGNATURES = {
     "pp_i3d_input": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "pp_maxpool3d_same": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_int] * 11 + [c_void_p]),
     "pp_mean_thw": (c_int, [c_void_p, c_int, c_void_p, c_int, c_long, c_int, c_void_p]),
+    "pp_cutie_topk_readout": (c_int, [c_void_p, c_void_p, c_void_p, c_long] + [c_int] * 3 + [c_void_p, c_void_p] + [c_int] * 3 +
+                              [c_void_p] * 4),
+    "pp_cutie_frame_in": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "pp_cutie_labels": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
 }
 
 _lib = None

@@ -1073,3 +1073,65 @@ def resize_flow(flows, size):
                                               _p(yo, torch.int32), _p(ya), _stream()), "pp_resize_flow_linear_cv")
     _count(1)
     return out
+
+
+# ---------------------------------------------------------------- Cutie mask tracker (web-demos/hugging_face/tracker)
+CUTIE_TOPK_MAX = 32
+
+
+def cutie_topk_readout(mem_key, mem_shrink, mem_value, n_frames, fifo_head, fifo_cap, qk, qe, top_k=30, num_objects=None,
+                       out=None, want_selection=False):
+    """The working-memory read of MemoryManager.read at top_k (memory_manager.py:160-187): similarity, top-k, softmax and
+    the value gather in one pass over ring buffers mem_key [slots*HW,64], mem_shrink [slots*HW], mem_value
+    [objects,slots*HW,256] (slots = 1 + fifo_cap; pp_cutie_topk_readout in include/propainter_b200.h) for query keys /
+    selections qk, qe [64,HW].  Returns out [num_objects,HW,256] (pixel-major), plus (sel_idx [HW,top_k] int32,
+    sel_w [HW,top_k]) when want_selection."""
+    HW = qk.shape[-1]
+    if qk.shape != (64, HW) or qe.shape != (64, HW):
+        raise RuntimeError(f"cutie_topk_readout: qk / qe must be [64,HW], got {tuple(qk.shape)} / {tuple(qe.shape)}")
+    slots = 1 + fifo_cap
+    if mem_key.shape != (slots * HW, 64) or mem_shrink.numel() != slots * HW or mem_value.shape[1:] != (slots * HW, 256):
+        raise RuntimeError("cutie_topk_readout: ring buffers do not match 1 + fifo_cap slots of HW tokens")
+    if not 1 <= top_k <= CUTIE_TOPK_MAX:
+        raise RuntimeError(f"cutie_topk_readout: top_k={top_k} outside [1, {CUTIE_TOPK_MAX}]")
+    nobj = mem_value.shape[0] if num_objects is None else num_objects
+    if mem_value.stride(2) != 1 or mem_value.stride(1) != 256:
+        raise RuntimeError("cutie_topk_readout: mem_value rows must be dense")
+    if out is None:
+        out = torch.empty(nobj, HW, 256, device=qk.device, dtype=torch.float32)
+    sel_idx = sel_w = None
+    if want_selection:
+        sel_idx = torch.empty(HW, top_k, device=qk.device, dtype=torch.int32)
+        sel_w = torch.empty(HW, top_k, device=qk.device, dtype=torch.float32)
+    check(_lib.lib().pp_cutie_topk_readout(_p(_dense(mem_key)), _p(_dense(mem_shrink)), _p(mem_value), mem_value.stride(0),
+                                           n_frames, fifo_head, fifo_cap, _p(_dense(qk)), _p(_dense(qe)), HW, nobj, top_k,
+                                           _p(_dense(out)), _p(sel_idx, torch.int32), _p(sel_w), _stream()),
+          "pp_cutie_topk_readout")
+    _count(1)
+    return (out, sel_idx, sel_w) if want_selection else out
+
+
+def cutie_frame_in(frame_u8, out=None):
+    """uint8 frame [H,W,3] on the device -> the normalised, zero-padded network input [1,3,Hp,Wp] (multiples of 16)"""
+    if frame_u8.dtype != torch.uint8 or frame_u8.dim() != 3 or frame_u8.shape[-1] != 3:
+        raise RuntimeError(f"cutie_frame_in: expected uint8 [H,W,3], got {frame_u8.dtype} {tuple(frame_u8.shape)}")
+    H, W, _ = frame_u8.shape
+    Hp, Wp = -(-H // 16) * 16, -(-W // 16) * 16
+    if out is None:
+        out = torch.empty(1, 3, Hp, Wp, device=frame_u8.device, dtype=torch.float32)
+    check(_lib.lib().pp_cutie_frame_in(_p(_dense(frame_u8), torch.uint8), _p(_dense(out)), H, W, _stream()), "pp_cutie_frame_in")
+    _count(1)
+    return out
+
+
+def cutie_labels(prob, lut, H, W, out=None):
+    """padded probabilities [K,Hp,Wp] -> uint8 labels [H,W]: argmax, unpad, then lut[K] (uint8, on the device)"""
+    K = prob.shape[0]
+    if prob.shape[1:] != (-(-H // 16) * 16, -(-W // 16) * 16) or lut.numel() != K or lut.dtype != torch.uint8:
+        raise RuntimeError(f"cutie_labels: prob {tuple(prob.shape)} / lut {tuple(lut.shape)} do not fit {H}x{W}")
+    if out is None:
+        out = torch.empty(H, W, device=prob.device, dtype=torch.uint8)
+    check(_lib.lib().pp_cutie_labels(_p(_dense(prob)), K, _p(_dense(lut), torch.uint8), _p(_dense(out), torch.uint8), H, W,
+                                     _stream()), "pp_cutie_labels")
+    _count(1)
+    return out

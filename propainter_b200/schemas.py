@@ -204,3 +204,137 @@ def generator_schema(depths=8, hidden=512, channel=128):
         S.linear(p + "mlp.fc1.0", hidden, 1960)
         S.linear(p + "mlp.fc2.1", 1960, hidden, gain=0.5)
     return S
+
+
+# ---------------------------------------------------------------------------------------------------------------- Cutie
+# The web demo's mask tracker (web-demos/hugging_face/tracker/model/cutie.py:18-45 at tracker/config CONFIG), pinned by
+# tests/golden/state_dict_manifest_cutie.json: resnet.py:38-121 (the two ResNets, through layer3), big_modules.py,
+# modules.py, group_modules.py, channel_attn.py, transformer/*.py and aux_modules.py (the aux head is kept so that
+# cutie-base-mega.pth loads strict; inference does not use it).
+def _bn(S, p, c, lo=0.4, hi=0.9):
+    S.add(p + ".weight", (c,), init=("uniform", lo, hi))
+    S.add(p + ".bias", (c,), init=("normal", 0.1))
+    S.add(p + ".running_mean", (c,), kind="buffer", init=("normal", 0.1))
+    S.add(p + ".running_var", (c,), kind="buffer", init=("uniform", 0.5, 2.0))
+    S.add(p + ".num_batches_tracked", (), kind="buffer", dtype=torch.int64, init=("zeros",))
+
+
+def _resnet(S, p, cin, bottleneck, blocks, layer_names):
+    """ResNet.__init__ / _make_layer (resnet.py:86-121) for layer1..layer3: bias-free convs (Kaiming-normal), BatchNorm2d"""
+    S.conv(p + ".conv1", cin, 64, 7, bias=False, gain=2 ** 0.5)
+    _bn(S, p + ".bn1", 64)
+    inplanes = 64
+    for name, planes, n, stride in zip(layer_names, (64, 128, 256), blocks, (1, 2, 2)):
+        out = planes * (4 if bottleneck else 1)
+        for b in range(n):
+            q = f"{p}.{name}.{b}"
+            if bottleneck:
+                S.conv(q + ".conv1", inplanes, planes, 1, bias=False, gain=2 ** 0.5)
+                _bn(S, q + ".bn1", planes)
+                S.conv(q + ".conv2", planes, planes, 3, bias=False, gain=2 ** 0.5)
+                _bn(S, q + ".bn2", planes)
+                S.conv(q + ".conv3", planes, out, 1, bias=False, gain=2 ** 0.5)
+                _bn(S, q + ".bn3", out, 0.2, 0.5)
+            else:
+                S.conv(q + ".conv1", inplanes, planes, 3, bias=False, gain=2 ** 0.5)
+                _bn(S, q + ".bn1", planes)
+                S.conv(q + ".conv2", planes, planes, 3, bias=False, gain=2 ** 0.5)
+                _bn(S, q + ".bn2", planes, 0.2, 0.5)
+            if b == 0 and (stride != 1 or inplanes != out):
+                S.conv(q + ".downsample.0", inplanes, out, 1, bias=False, gain=2 ** 0.5)
+                _bn(S, q + ".downsample.1", out, 0.2, 0.5)
+            inplanes = out
+
+
+def _ca_block(S, p, dim):
+    """CAResBlock (channel_attn.py:7-25) with in_dim == out_dim: two 3x3 convs + the ECA conv1d (k = 5 at 256 channels)"""
+    S.conv(p + ".conv1", dim, dim, 3)
+    S.conv(p + ".conv2", dim, dim, 3)
+    S.add(p + ".conv.weight", (1, 1, 5), init=("normal", 5 ** -0.5))
+
+
+def _fusion(S, p, x_dim, g_dim, out_dim):
+    """GroupFeatureFusionBlock (group_modules.py:107-118)"""
+    S.conv(p + ".distributor.x_transform", x_dim, out_dim, 1)
+    S.conv(p + ".distributor.g_transform", g_dim, out_dim, 1)
+    _ca_block(S, p + ".block1", out_dim)
+    _ca_block(S, p + ".block2", out_dim)
+
+
+def _mha(S, p, dim):
+    """nn.MultiheadAttention(dim, heads, batch_first=True): packed in-projection + out_proj"""
+    S.add(p + ".in_proj_weight", (3 * dim, dim), init=("normal", dim ** -0.5))
+    S.add(p + ".in_proj_bias", (3 * dim,), init=("normal", 0.02))
+    S.linear(p + ".out_proj", dim, dim)
+
+
+def cutie_pe_inv_freq(dim=256, temperature=128):
+    """PositionalEncoding.inv_freq (transformer/positional_encoding.py:21-23), a persistent buffer of the state_dict"""
+    d = int(-(-dim // 4) * 2)
+    return (1.0 / (temperature ** (torch.arange(0, d, 2).float() / d))).tolist()
+
+
+CUTIE_DIMS = dict(pixel_dim=256, key_dim=64, value_dim=256, sensory_dim=256, embed_dim=256, ms_dims=(1024, 512, 256),
+                  num_queries=16, num_heads=8, num_blocks=3, ff_dim=2048, up_dims=(256, 128, 128))
+
+
+def cutie_schema():
+    """CUTIE(cfg) (tracker/model/cutie.py:18-45) at tracker/config CONFIG, multi-object, in its state_dict order"""
+    d = CUTIE_DIMS
+    E, V, SD, K = d["embed_dim"], d["value_dim"], d["sensory_dim"], d["key_dim"]
+    S = Schema()
+    _resnet(S, "pixel_encoder", 3, True, (3, 4, 6), ("res2", "layer2", "layer3"))
+    S.conv("pix_feat_proj", 1024, d["pixel_dim"], 1)
+    S.conv("key_proj.pix_feat_proj", 1024, d["pixel_dim"], 1)
+    S.conv("key_proj.key_proj", d["pixel_dim"], K, 3)
+    S.conv("key_proj.d_proj", d["pixel_dim"], 1, 3)
+    S.conv("key_proj.e_proj", d["pixel_dim"], K, 3)
+    _resnet(S, "mask_encoder", 5, False, (2, 2, 2), ("layer1", "layer2", "layer3"))
+    _fusion(S, "mask_encoder.fuser", d["pixel_dim"], 256, V)
+    S.conv("mask_encoder.sensory_update.transform", V + SD, SD * 3, 3)
+    u0, u1, u2 = d["up_dims"]
+    S.conv("mask_decoder.sensory_update.g16_conv", u0, SD, 1)
+    S.conv("mask_decoder.sensory_update.g8_conv", u1, SD, 1)
+    S.conv("mask_decoder.sensory_update.g4_conv", u2 + 1, SD, 1)
+    S.conv("mask_decoder.sensory_update.transform", SD + SD, SD * 3, 3)
+    S.conv("mask_decoder.decoder_feat_proc.transforms.0", d["ms_dims"][1], u0, 1)
+    S.conv("mask_decoder.decoder_feat_proc.transforms.1", d["ms_dims"][2], u1, 1)
+    S.conv("mask_decoder.up_16_8.out_conv.downsample", u0, u1, 1)
+    S.conv("mask_decoder.up_16_8.out_conv.conv1", u0, u1, 3)
+    S.conv("mask_decoder.up_16_8.out_conv.conv2", u1, u1, 3)
+    S.conv("mask_decoder.up_8_4.out_conv.conv1", u1, u2, 3)
+    S.conv("mask_decoder.up_8_4.out_conv.conv2", u2, u2, 3)
+    S.conv("mask_decoder.pred", u2, 1, 3)
+    _fusion(S, "pixel_fuser.fuser", d["pixel_dim"], V, E)
+    S.conv("pixel_fuser.sensory_compress", SD + 2, V, 1)
+    t = "object_transformer"
+    Q = d["num_queries"]
+    S.add(t + ".query_init.weight", (Q, E), init=("normal", 1.0))
+    S.add(t + ".query_emb.weight", (Q, E), init=("normal", 1.0))
+    S.linear(t + ".summary_to_query_init", E, E)
+    S.linear(t + ".summary_to_query_emb", E, E)
+    S.conv(t + ".pixel_init_proj", E, E, 1)
+    S.conv(t + ".pixel_emb_proj", E, E, 1)
+    S.add(t + ".spatial_pe.inv_freq", (E // 4,), kind="buffer", init=("const", cutie_pe_inv_freq(E)))
+    for b in range(d["num_blocks"]):
+        q = f"{t}.blocks.{b}"
+        _mha(S, q + ".read_from_pixel.cross_attn", E)
+        S.affine(q + ".read_from_pixel.norm", E)
+        _mha(S, q + ".self_attn.self_attn", E)
+        S.affine(q + ".self_attn.norm", E)
+        S.linear(q + ".ffn.linear1", E, d["ff_dim"])
+        S.linear(q + ".ffn.linear2", d["ff_dim"], E)
+        S.affine(q + ".ffn.norm", E)
+        _mha(S, q + ".read_from_query.cross_attn", E)
+        _ca_block(S, q + ".pixel_ffn.conv", E)
+    for i in range(d["num_blocks"] + 1):
+        S.conv(f"{t}.mask_pred.{i}.1", E, 1, 1)
+    s = "object_summarizer"
+    S.add(s + ".pos_enc.inv_freq", (E // 4,), kind="buffer", init=("const", cutie_pe_inv_freq(E)))
+    S.linear(s + ".input_proj", V, E)
+    S.linear(s + ".feature_pred.0", E, E)
+    S.linear(s + ".feature_pred.2", E, E)
+    S.linear(s + ".weights_pred.0", E, E)
+    S.linear(s + ".weights_pred.2", E, Q)
+    S.conv("aux_computer.sensory_aux.projection", SD, E + 1, 1)
+    return S
