@@ -288,6 +288,10 @@ int pp_bias_act_pre(const float* x, int ld_x, const float* bias, const float* pr
  * bias, pre, res and the arithmetic stay fp32.  The epilogue of RAFT's half-precision refinement-loop convs. */
 int pp_bias_act_f16(const void* x, int ld_x, int x_f16, const float* bias, const float* pre, int ld_pre, const float* res, int ld_res,
                     void* out, int ld_out, int out_f16, long n_pix, int C, int act, float slope, int post_relu, cudaStream_t stream);
+/* pp_bias_act with fp16 x, residual res (may be NULL) and out, 8-byte aligned rows; bias and arithmetic fp32, out rounded
+   to nearest once.  Returns PP_ERR_ALIGN / PP_ERR_SHAPE like pp_bias_act_f16. */
+int pp_bias_act_f16_res(const void* x, int ld_x, const float* bias, const void* res, int ld_res, void* out, int ld_out, long n_pix,
+                        int C, int act, float slope, int post_relu, cudaStream_t stream);
 
 /* nn.InstanceNorm2d(affine=False, eps) of the RAFT feature encoder (RAFT/extractor.py:18-21,125,168-192) on channels-last
  * maps x [n][HW][C]: out = post(relu?((x - mean) * rstd) + res), statistics per (sample, channel), biased variance,

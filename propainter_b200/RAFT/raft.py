@@ -131,18 +131,38 @@ class RAFT(ParamNet):
         """BasicEncoder.forward extractor.py:168-192.  fnet: conv -> InstanceNorm -> ReLU with the norm, the ReLU and the
         block's `relu(x + y)` as one pp_instance_norm call on the raw conv output (the conv bias cancels under the
         per-channel mean subtraction, so it is not even added).  cnet: eval BatchNorm folded into the conv; bias, ReLU
-        and the residual add + ReLU are one pp_bias_act pass."""
+        and the residual add + ReLU are one pp_bias_act pass.
+        cnet under config.half_convs() (CUDA tensors) runs on fp16 operands: frames rounded to fp16 and padded to 8 channels
+        (zero weight columns), fp16 weights, cuDNN convs with fp32 accumulation writing fp16, pp_bias_act epilogues on fp16
+        maps with an fp16 residual (fp32 arithmetic, each map rounded once); conv2 is widened on store, so the result is
+        fp32 [n,256,h,w] channels_last either way and `net` / `inp` stay fp32.  fnet stays on TF32: every InstanceNorm it
+        runs is held to the fp32 kernel's float64 bound, and on fp16 maps its outputs land up to ~1.4e3 times outside it."""
         inst = p == "fnet"
+        half = not inst and x.is_cuda and config.half_convs()
 
-        def cn(key, bn, t, stride=1, pad=1, relu=True, res=None):
+        def wb(key, bn=None, cin_pad=None):
+            if not half:
+                return self._wb(key, bn)
+
+            def build():
+                w, b = self._wb(key, bn)
+                return cl(pad_in_channels(w, cin_pad) if cin_pad else w).half(), b
+            return self.packed(f"f16:{key}:{cin_pad}", build)
+
+        def cn(key, bn, t, stride=1, pad=1, relu=True, res=None, cin_pad=None):
             if inst:
                 w, _ = self._wb(key)
                 y = as_pm(F.conv2d(t, w, None, stride=stride, padding=pad))
                 return as_nchw(ops.instance_norm(y, relu=relu, res=None if res is None else as_pm(res),
                                                  post_relu=res is not None, out=y))
-            return conv(t, self._wb(key, bn), stride, pad, act="relu" if relu else "none", res=res, post_relu=res is not None)
+            return conv(t, wb(key, bn, cin_pad), stride, pad, act="relu" if relu else "none", res=res, post_relu=res is not None)
 
-        x = cn(p + ".conv1", p + ".norm1", x, 2, 3)
+        if half:
+            n, _, H, W = x.shape
+            x16 = torch.zeros(n, H, W, 8, device=x.device, dtype=torch.float16)
+            x16[..., :3].copy_(as_pm(x))
+            x = as_nchw(x16)
+        x = cn(p + ".conv1", p + ".norm1", x, 2, 3, cin_pad=8 if half else None)
         for li, stride in ((1, 1), (2, 2), (3, 2)):
             for bi in (0, 1):
                 q = f"{p}.layer{li}.{bi}"
@@ -151,6 +171,9 @@ class RAFT(ParamNet):
                 if s != 1:
                     x = cn(q + ".downsample.0", q + ".norm3", x, s, 0, relu=False)
                 x = cn(q + ".conv2", q + ".norm2", y, 1, 1, res=x)              # relu(x + relu(norm(conv2(y))))
+        if half:
+            m, _, h, w = x.shape
+            return conv(x, wb(p + ".conv2"), out=as_nchw(torch.empty(m, h, w, 256, device=x.device)))
         return conv(x, self._wb(p + ".conv2"))
 
     def _encode_small(self, p, x):

@@ -111,6 +111,8 @@ SIGNATURES = {
                                 c_int, c_void_p]),
     "pp_bias_act_f16": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_long, c_int,
                                 c_int, c_float, c_int, c_void_p]),
+    "pp_bias_act_f16_res": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_long, c_int, c_int, c_float, c_int,
+                                    c_void_p]),
     "pp_pool_depthwise": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "pp_add_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_long, c_int, c_float, c_void_p]),
     "pp_pool_depthwise_f16": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,

@@ -33,6 +33,10 @@ HALF_OPERANDS   RAFT's refinement-loop convs (convc1, convc2, convf2, the motion
                 torch.backends.cuda.matmul.allow_tf32, CUDA tensors), so a strict-fp32 run stays strict.
                 Where cuDNN may use TF32 (half_convs) it also runs the per-step convs of the two recurrent propagation
                 scans (plan 0 of UMMA_CONV) on the fp16 instance of pp_conv2d_umma; their states stay fp32.
+                There it also runs two clip encoders on fp16 operands: the generator's frame encoder (fp16 input, weights
+                and maps, the grouped layers' inputs written into their group slots by the previous epilogue) and RAFT's
+                context encoder cnet (pp_bias_act epilogues with an fp16 residual); both widen their last conv's output
+                to fp32, so the encoder features, `net` and `inp` stay fp32.  RAFT's feature encoder fnet stays TF32.
                 Environment: PP_HALF_OPERANDS=0|1.
 AUTOTUNE        time numerically equivalent plans of a step once per shape during warm-up and keep the faster
                 (propainter_b200/autotune.py): grouped conv vs per-group dense convs, conv + pp_bias_act vs cuDNN's fused

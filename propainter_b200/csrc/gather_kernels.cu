@@ -575,9 +575,10 @@ extern "C" int pp_sc_fold_f16(const void* cols, long ldc, const float* bmap, voi
 // separate bias add_ kernel, the activation kernel, the residual add and (with a strided `out`) the torch.cat that
 // would place the result into a concat buffer.  act: 0 none, 1 relu, 2 leaky(slope), 3 sigmoid, 4 tanh; bias / res may
 // be NULL; post_relu applies a final ReLU (residual blocks).  out may alias x.  TX / TO: fp32 or fp16 rows of x / out
-// (the half-operand convs of RAFT's refinement loop); bias, pre, res and the arithmetic stay fp32.
-template <typename TX, typename TO>
-__global__ void __launch_bounds__(256) k_bias_act(const TX* x, int ld_x, const float* __restrict__ bias, const float* res,
+// (the half-operand convs of RAFT's refinement loop); TR: fp32 or fp16 rows of res (the residual stream of RAFT's
+// half-operand context encoder); bias, pre and the arithmetic stay fp32.
+template <typename TX, typename TO, typename TR = float>
+__global__ void __launch_bounds__(256) k_bias_act(const TX* x, int ld_x, const float* __restrict__ bias, const TR* res,
                                                   int ld_res, TO* out, int ld_out, long n_pix, int C, int act, float slope,
                                                   int post_relu, const float* __restrict__ pre = nullptr, int ld_pre = 0) {
   const int c4n = C >> 2;
@@ -604,7 +605,7 @@ __global__ void __launch_bounds__(256) k_bias_act(const TX* x, int ld_x, const f
     r[k] = t;
   }
   if (res != nullptr) {
-    const float4 q = *reinterpret_cast<const float4*>(res + pix * ld_res + c);
+    const float4 q = pp_ld4(res + pix * ld_res + c);
     r[0] += q.x; r[1] += q.y; r[2] += q.z; r[3] += q.w;
   }
   if (post_relu) {
@@ -669,6 +670,20 @@ extern "C" int pp_bias_act_f16(const void* x, int ld_x, int x_f16, const float* 
   else
     k_bias_act<float, float><<<nb, 256, 0, stream>>>((const float*)x, ld_x, bias, res, ld_res, (float*)out, ld_out, n_pix, C, act,
                                                      slope, post_relu, pre, ld_pre);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+
+// pp_bias_act on fp16 rows throughout: x, the residual res (may be NULL) and out are fp16 (8-byte aligned rows), bias and the
+// arithmetic fp32, out rounded once.  The residual blocks of RAFT's half-operand context encoder.
+extern "C" int pp_bias_act_f16_res(const void* x, int ld_x, const float* bias, const void* res, int ld_res, void* out, int ld_out,
+                                   long n_pix, int C, int act, float slope, int post_relu, cudaStream_t stream) {
+  if (C % 4 || ld_x % 4 || ld_out % 4 || (res && ld_res % 4)) return PP_ERR_ALIGN;
+  if (((uintptr_t)x & 7) || ((uintptr_t)out & 7) || ((uintptr_t)bias & 15) || ((uintptr_t)res & 7)) return PP_ERR_ALIGN;
+  if (ld_x < C || ld_out < C || (res && ld_res < C) || act < 0 || act > 4) return PP_ERR_SHAPE;
+  if (n_pix <= 0) return PP_OK;
+  k_bias_act<__half, __half, __half><<<pp_blocks(n_pix * (C / 4), 256), 256, 0, stream>>>(
+      (const __half*)x, ld_x, bias, (const __half*)res, ld_res, (__half*)out, ld_out, n_pix, C, act, slope, post_relu);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }

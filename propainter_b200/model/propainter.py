@@ -46,6 +46,10 @@ class InpaintGenerator(ParamNet):
             return cl(w), self.P[key + ".bias"].contiguous()
         return self.packed(f"wb:{key}:{cin_pad}", build)
 
+    def _wb16(self, key, cin_pad=None):
+        """_wb with an fp16 weight (the bias stays fp32) for the half-operand convs"""
+        return self.packed(f"f16:{key}:{cin_pad}", lambda: (self._wb(key, cin_pad)[0].half(), self._wb(key, cin_pad)[1]))
+
     def _wb_group(self, key, j, g):
         """(weight, bias) of group j of a grouped conv, as a dense conv."""
         def build():
@@ -113,6 +117,54 @@ class InpaintGenerator(ParamNet):
                 out = autotune.pick(("enc_group", i, tuple(x0.shape), tuple(o.shape)), (grouped, per_group), x0, o)
         return out
 
+    def _encoder_half(self, x):
+        """_encoder on fp16 operands (config.half_convs): x [n,8,H,W] fp16 channels_last; fp16 weights and maps, cuDNN convs
+        with fp32 accumulation, bias + LeakyReLU in fp32 by pp_bias_act, each map rounded once to fp16; layers.16 is widened
+        on store, so the result is fp32 [n,128,h,w] channels_last as on the fp32 path."""
+        L = dict(act="leaky", slope=0.2)
+        out = conv(x, self._wb16("encoder.layers.0", 8), 2, 1, **L)
+        out = conv(out, self._wb16("encoder.layers.2"), 1, 1, **L)
+        out = conv(out, self._wb16("encoder.layers.4"), 2, 1, **L)
+        x0 = as_pm(conv(out, self._wb16("encoder.layers.6"), 1, 1, **L))                # [n,h,w,256]
+        raw = as_pm(F.conv2d(as_nchw(x0), self._wb16("encoder.layers.8")[0], None, 1, 1))  # layers.8 before its epilogue
+        return autotune.pick(("enc_group", torch.float16, tuple(x0.shape), tuple(raw.shape)),
+                             (lambda a, b: self._enc_groups_half(a, b, True), lambda a, b: self._enc_groups_half(a, b, False)),
+                             x0, raw)
+
+    def _enc_groups_half(self, x0, raw, interleaved):
+        """layers.8's epilogue and the grouped layers 10 / 12 / 14 / 16 on fp16 operands.  Group j of a layer with g groups
+        reads [x0_j | o_j] (a = 256/g channels of x0, b of the previous output o).  These inputs are not concatenated: each
+        layer's input buffer is allocated in the layout its conv reads -- interleaved [n,h,w,g,a+b] for one grouped conv, or
+        group-major [g][n,h,w,a+b] for g dense convs (the per-group plan) -- x0 is copied into its slots once, and the
+        previous layer's bias + LeakyReLU (pp_bias_act, one call per group slot it reaches) writes o into the rest."""
+        n, h, w, c0 = x0.shape
+        pieces, bias = [(raw, 0)], self.P["encoder.layers.8.bias"]        # raw conv outputs and their first output channel
+        for i, g in ((10, 2), (12, 4), (14, 8), (16, 1)):
+            key = f"encoder.layers.{i}"
+            a, b = c0 // g, bias.shape[0] // g
+            if interleaved:
+                buf = torch.empty(n, h, w, g, a + b, device=x0.device, dtype=torch.float16)
+                buf[..., :a].copy_(x0.view(n, h, w, g, a))
+                slots = [buf[..., k, :] for k in range(g)]
+            else:
+                buf = torch.empty(g, n, h, w, a + b, device=x0.device, dtype=torch.float16)
+                buf[..., :a].copy_(x0.view(n, h, w, g, a).permute(3, 0, 1, 2, 4))
+                slots = list(buf)
+            for y, cs in pieces:                   # output channel c of the previous layer -> slot c // b, column a + c % b
+                for k in range(cs // b, (cs + y.shape[-1] - 1) // b + 1):
+                    lo, hi = max(cs, k * b), min(cs + y.shape[-1], (k + 1) * b)
+                    ops.bias_act(y[..., lo - cs:hi - cs], bias[lo:hi], "leaky", 0.2,
+                                 out=slots[k][..., a + lo - k * b:a + hi - k * b])
+            wt, bias = self._wb16(key)
+            co = wt.shape[0] // g
+            if interleaved:
+                pieces = [(as_pm(F.conv2d(as_nchw(buf.view(n, h, w, -1)), wt, None, 1, 1, 1, g)), 0)]
+            else:
+                wg = [self.packed(f"f16:wbg:{key}:{j}", lambda j=j: self._wb_group(key, j, g)[0].half()) for j in range(g)]
+                pieces = [(as_pm(F.conv2d(as_nchw(slots[j]), wg[j], None, 1, 1)), j * co) for j in range(g)]
+        (y, _), = pieces
+        return as_nchw(ops.bias_act(y, bias, "leaky", 0.2, out=torch.empty(y.shape, device=y.device)))   # widened to fp32
+
     def _decoder(self, x):
         """x [lt,128,h,w] channels_last -> the pre-tanh image [lt,3,4h,4w], fp32.  fp16 x (half-operand trunk): fp16 weights
         and maps, fp32 accumulation and epilogues; decoder.6 gets a zero fourth output channel so that its bias is added as
@@ -123,10 +175,9 @@ class InpaintGenerator(ParamNet):
             x = conv(x, self._wb("decoder.2"), 1, 1, **L)
             x = conv(up2(x), self._wb("decoder.4.conv"), 1, 1, **L)
             return conv(x, self._wb("decoder.6"), 1, 1)
-        wb16 = lambda k: self.packed("f16:" + k, lambda: (self._wb(k)[0].half(), self._wb(k)[1]))
-        x = conv(up2(x), wb16("decoder.0.conv"), 1, 1, **L)
-        x = conv(x, wb16("decoder.2"), 1, 1, **L)
-        x = conv(up2(x), wb16("decoder.4.conv"), 1, 1, **L)
+        x = conv(up2(x), self._wb16("decoder.0.conv"), 1, 1, **L)
+        x = conv(x, self._wb16("decoder.2"), 1, 1, **L)
+        x = conv(up2(x), self._wb16("decoder.4.conv"), 1, 1, **L)
         w6, b6 = self.packed("f16:decoder.6", lambda: (cl(F.pad(self.P["decoder.6.weight"], (0, 0, 0, 0, 0, 0, 0, 1))).half(),
                                                        F.pad(self.P["decoder.6.bias"], (0, 1)).contiguous()))
         n, _, H, W = x.shape
@@ -384,6 +435,11 @@ class InpaintGenerator(ParamNet):
 
     def _encode_frames(self, fr, mi, mu):
         n, _, H, W = fr.shape
+        if fr.is_cuda and config.half_convs():
+            x = torch.zeros(n, H, W, 8, device=fr.device, dtype=torch.float16)
+            for c0, t in ((0, fr), (3, mi), (4, mu)):
+                x[..., c0:c0 + t.shape[1]].copy_(as_pm(t))
+            return self._encoder_half(as_nchw(x))
         x = torch.cat([fr, mi, mu, fr.new_zeros(n, 3, H, W)], 1).contiguous(memory_format=torch.channels_last)
         return self._encoder(x).contiguous(memory_format=torch.channels_last)
 

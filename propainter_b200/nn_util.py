@@ -53,8 +53,8 @@ def conv(x, wb, stride=1, padding=0, dilation=1, groups=1, act="none", slope=0.0
     a separate bias add_, ATen one kernel each for the activation, the residual add and the torch.cat).  `res` / `out`
     are NCHW-logical channels_last views; `pre` (same kind of view) is added before the activation (a conv share computed
     ahead of time).  Plain conv+bias+ReLU may instead run as cuDNN's fused conv-bias-ReLU when
-    that measures faster for the shape (autotune.pick).  Outputs whose channel count is not a multiple of 4
-    (2/3-channel heads) keep the library epilogue."""
+    that measures faster for the shape (autotune.pick; not for fp16 x, whose bias stays fp32).  Outputs whose channel
+    count is not a multiple of 4 (2/3-channel heads) keep the library epilogue."""
     w, b = wb
     st, pd, dl = _pair(stride), _pair(padding), _pair(dilation)
     if not (config.FUSED_EPILOGUE and w.shape[0] % 4 == 0):
@@ -76,10 +76,11 @@ def conv(x, wb, stride=1, padding=0, dilation=1, groups=1, act="none", slope=0.0
                          out=None if out is None else out.permute(0, 2, 3, 1), pre=None if pre is None else pre.permute(0, 2, 3, 1))
         return as_nchw(o)
 
-    if act == "relu" and res is None and out is None and pre is None and not post_relu and config.AUTOTUNE:
+    if (act == "relu" and res is None and out is None and pre is None and not post_relu and config.AUTOTUNE
+            and (b is None or x.dtype == b.dtype)):
         def fused(x):
             return torch.cudnn_convolution_relu(x, w, b, st, pd, dl, groups).contiguous(memory_format=torch.channels_last)
-        return autotune.pick(("conv_relu", tuple(x.shape), tuple(w.shape), st, pd, dl, groups), (own, fused), x)
+        return autotune.pick(("conv_relu", tuple(x.shape), tuple(w.shape), st, pd, dl, groups, x.dtype), (own, fused), x)
     return own(x)
 
 

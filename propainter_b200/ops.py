@@ -586,11 +586,22 @@ ACT = {"none": 0, "relu": 1, "leaky": 2, "sigmoid": 3, "tanh": 4}
 def bias_act(x_pm, bias=None, act="none", slope=0.0, res=None, post_relu=False, out=None, pre=None):
     """out = post(act(x + bias + pre) + res) on pixel-major views [..., C] (unit channel stride, dense over pixels; x / pre /
     res / out may each be a channel slice of a wider buffer).  out=None -> in place on x_pm.  Returns out.  x_pm and out may
-    be fp16 (RAFT's half-precision refinement convs); bias / pre / res and the arithmetic are fp32."""
+    be fp16 (RAFT's half-precision refinement convs); bias / pre and the arithmetic are fp32.  res is fp32, or fp16 with fp16
+    x and out (the residual blocks of RAFT's half-operand context encoder)."""
     C = x_pm.shape[-1]
     out = x_pm if out is None else out
     if out.shape != x_pm.shape or (res is not None and res.shape != x_pm.shape) or (pre is not None and pre.shape != x_pm.shape):
         raise RuntimeError("bias_act: shape mismatch")
+    if res is not None and res.dtype == torch.float16:
+        if x_pm.dtype != torch.float16 or out.dtype != torch.float16 or pre is not None:
+            raise RuntimeError("bias_act: an fp16 residual needs fp16 x and out and no pre")
+        xp, ldx = _pm(x_pm, torch.float16)
+        op, ldo = _pm(out, torch.float16)
+        rp, ldr = _pm(res, torch.float16)
+        check(_lib.lib().pp_bias_act_f16_res(xp, ldx, _p(bias), rp, ldr, op, ldo, x_pm.numel() // C, C, ACT[act], float(slope),
+                                             int(bool(post_relu)), _stream()), "pp_bias_act_f16_res")
+        _count(1)
+        return out
     if torch.float16 in (x_pm.dtype, out.dtype):
         if not {x_pm.dtype, out.dtype} <= {torch.float16, torch.float32}:
             raise RuntimeError(f"bias_act: x / out must be fp32 or fp16, got {x_pm.dtype} / {out.dtype}")
