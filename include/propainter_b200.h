@@ -433,6 +433,16 @@ int pp_cutie_frame_in(const uint8_t* frame, float* out, int H, int W, cudaStream
 /* torch.argmax over K probability channels [K][Hp][Wp] (padded as pp_cutie_frame_in), unpad and the MaskMapper remapping
  * lut[K] (base_tracker.py:79-87) -> uint8 labels [H][W]. */
 int pp_cutie_labels(const float* prob, int K, const uint8_t* lut, uint8_t* out, int H, int W, cudaStream_t stream);
+/* The tracking preview: BaseTracker.track's painter loop (base_tracker.py:90-95) over a clip.  Every non-zero id k of
+ * labels uint8 [T][H][W] present in a frame, in ascending order, goes through mask_painter (tools/painter.py:137-157,
+ * contour width 3): fill with palette row k + 1 in float64 (frames * alpha[1] + row * alpha[0], truncated; alpha[1] is
+ * 1 - alpha as the caller computes it), then palette row 1 on its contour.  frames uint8 [T][H][W][3] -> out (may be
+ * frames); palette uint8 [n_colors][3], ids with k + 1 >= n_colors are left unpainted.  Byte-exact with the reference
+ * (the rules are pp_paint_* in pp_elem.cuh).  Caller-owned workspace of pp_mask_paint_workspace_bytes(T, H, W) bytes (0
+ * for an invalid shape), 4-byte aligned.  PP_ERR_SHAPE unless 1 <= T <= 65535, H, W >= 1 and n_colors >= 2. */
+size_t pp_mask_paint_workspace_bytes(int T, int H, int W);
+int pp_mask_paint_u8(const uint8_t* frames, const uint8_t* labels, const uint8_t* palette, int n_colors, const double* alpha,
+                     uint8_t* out, int T, int H, int W, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
 #ifdef __cplusplus
 }

@@ -157,6 +157,9 @@ SIGNATURES = {
                               [c_void_p] * 4),
     "pp_cutie_frame_in": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "pp_cutie_labels": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "pp_mask_paint_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "pp_mask_paint_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t,
+                                 c_void_p]),
 }
 
 _lib = None

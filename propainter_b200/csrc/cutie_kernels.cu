@@ -1,7 +1,8 @@
 // The web demo's Cutie mask tracker on sm_90a (web-demos/hugging_face/tracker): the fused top-k memory readout of the
 // working memory, and the frame / label passes at the two ends of a tracking step.  The networks' convolutions stay
-// cuDNN calls (propainter_b200/model/cutie.py).
+// cuDNN calls (propainter_b200/model/cutie.py).  And the tracking preview: the painted frames BaseTracker.track returns.
 #include <limits.h>
+#include "pp_elem.cuh"
 #include "pp_topk.cuh"
 #include "../../include/propainter_b200.h"
 
@@ -242,6 +243,150 @@ extern "C" int pp_cutie_labels(const float* prob, int K, const uint8_t* lut, uin
   const int Hp = (H + 15) / 16 * 16, Wp = (W + 15) / 16 * 16;
   const long n = (long)H * W;
   k_cutie_labels<<<pp_blocks(n, 256), 256, 0, stream>>>(prob, K, Hp, Wp, (Hp - H) / 2, (Wp - W) / 2, lut, out, H, W);
+  PP_LAUNCH_CHECK();
+  return PP_OK;
+}
+
+// ================================================================ tracking preview
+// BaseTracker.track's painter loop (base_tracker.py:90-95) over a whole clip, from the rules of pp_elem.cuh.  Pass 1
+// finds the per-(frame, object) maxima M: k_mask_paint_partial takes, per 32 x 32 tile, the maximum of v for each id of
+// pp_paint_candidates (none in most frames: then the block returns at once), k_mask_paint_maxima reduces the tiles and
+// sets M = 3 for every other id.  Pass 2 (k_mask_paint_u8) paints each pixel from its 7x7 label window.  Each block
+// stages its tile's labels with a 3-pixel halo in shared memory, -1 outside the frame.  Maxima in a fixed tree, no
+// atomics: the same bits on every run.
+#define MP_TILE 32
+#define MP_ROWS 8                                  // 32 x 8 threads, 4 rows of the tile each
+#define MP_THREADS (MP_TILE * MP_ROWS)
+#define MP_LD (MP_TILE + 6)
+#define MP_CANDS 16                                // >= the 11 ids that can reach pixel (0, 0)
+
+static inline long mp_tiles(int H, int W) { return (long)((H + MP_TILE - 1) / MP_TILE) * ((W + MP_TILE - 1) / MP_TILE); }
+
+__device__ void mp_stage(const uint8_t* __restrict__ lab, int H, int W, int y0, int x0, int* s) {
+  for (int i = threadIdx.y * MP_TILE + threadIdx.x; i < MP_LD * MP_LD; i += MP_THREADS) {
+    const int y = y0 - 3 + i / MP_LD, x = x0 - 3 + i % MP_LD;
+    s[i] = (y >= 0 && y < H && x >= 0 && x < W) ? lab[(long)y * W + x] : -1;
+  }
+}
+
+// pp_paint_candidates of one frame's pixel (0, 0), read from global memory by one thread
+__device__ int mp_candidates(const uint8_t* __restrict__ lab, int H, int W, int* out) {
+  int w[49];
+#pragma unroll
+  for (int i = 0; i < 49; ++i) {
+    const int y = i / 7 - 3, x = i % 7 - 3;
+    w[i] = (y >= 0 && y < H && x >= 0 && x < W) ? lab[(long)y * W + x] : -1;
+  }
+  return pp_paint_candidates(w + 24, 7, out);
+}
+
+// maximum over the block's threads, result valid in thread 0; red holds MP_THREADS / 32 floats
+__device__ float mp_block_max(float v, float* red) {
+  const int t = threadIdx.y * MP_TILE + threadIdx.x;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if ((t & 31) == 0) red[t >> 5] = v;
+  __syncthreads();
+  if (t == 0)
+    for (int i = 1; i < MP_THREADS / 32; ++i) v = fmaxf(v, red[i]);
+  __syncthreads();
+  return v;
+}
+
+__global__ void __launch_bounds__(MP_THREADS) k_mask_paint_partial(const uint8_t* __restrict__ labels, int H, int W, int tiles_x,
+                                                                   long ntiles, float* __restrict__ partial) {
+  __shared__ int s_lab[MP_LD * MP_LD];
+  __shared__ int s_cand[MP_CANDS], s_n;
+  __shared__ float s_red[MP_THREADS / 32];
+  const int f = blockIdx.y, t = threadIdx.y * MP_TILE + threadIdx.x;
+  const uint8_t* lab = labels + (long)f * H * W;
+  if (t == 0) s_n = mp_candidates(lab, H, W, s_cand);
+  __syncthreads();
+  const int n = s_n;
+  if (n == 0) return;
+  const int y0 = (blockIdx.x / tiles_x) * MP_TILE, x0 = (blockIdx.x % tiles_x) * MP_TILE;
+  mp_stage(lab, H, W, y0, x0, s_lab);
+  __syncthreads();
+  for (int j = 0; j < n; ++j) {
+    float m = 0.0f;
+    if (x0 + (int)threadIdx.x < W)
+      for (int r = threadIdx.y; r < MP_TILE && y0 + r < H; r += MP_ROWS)
+        m = fmaxf(m, pp_paint_dist(s_lab + (r + 3) * MP_LD + threadIdx.x + 3, MP_LD, s_cand[j]));
+    m = mp_block_max(m, s_red);
+    if (t == 0) partial[((long)f * ntiles + blockIdx.x) * MP_CANDS + j] = m;
+  }
+}
+
+__global__ void __launch_bounds__(MP_THREADS) k_mask_paint_maxima(const uint8_t* __restrict__ labels, int H, int W, long ntiles,
+                                                                  const float* __restrict__ partial, float* __restrict__ maxima) {
+  __shared__ int s_cand[MP_CANDS], s_n;
+  __shared__ float s_red[MP_THREADS / 32];
+  const int f = blockIdx.x, t = threadIdx.y * MP_TILE + threadIdx.x;
+  if (t == 0) s_n = mp_candidates(labels + (long)f * H * W, H, W, s_cand);
+  maxima[(long)f * 256 + t] = 3.0f;
+  __syncthreads();
+  for (int j = 0; j < s_n; ++j) {
+    float m = 0.0f;
+    for (long i = t; i < ntiles; i += MP_THREADS) m = fmaxf(m, partial[((long)f * ntiles + i) * MP_CANDS + j]);
+    m = mp_block_max(m, s_red);
+    if (t == 0) maxima[(long)f * 256 + s_cand[j]] = m;
+  }
+}
+
+// frames and out may be the same buffer: each thread reads a pixel before it writes it, and no other thread touches it
+__global__ void __launch_bounds__(MP_THREADS) k_mask_paint_u8(const uint8_t* frames, const uint8_t* __restrict__ labels,
+                                                              const uint8_t* __restrict__ palette, int n_colors, double alpha,
+                                                              double oma, const float* __restrict__ maxima, uint8_t* out, int H,
+                                                              int W, int tiles_x) {
+  __shared__ int s_lab[MP_LD * MP_LD];
+  __shared__ float s_max[256];
+  __shared__ uint8_t s_pal[257 * 3];
+  const int f = blockIdx.y, t = threadIdx.y * MP_TILE + threadIdx.x;
+  const long HW = (long)H * W;
+  const int y0 = (blockIdx.x / tiles_x) * MP_TILE, x0 = (blockIdx.x % tiles_x) * MP_TILE;
+  mp_stage(labels + f * HW, H, W, y0, x0, s_lab);
+  s_max[t] = maxima[(long)f * 256 + t];
+  for (int i = t; i < n_colors * 3; i += MP_THREADS) s_pal[i] = palette[i];
+  __syncthreads();
+  const int x = x0 + threadIdx.x;
+  if (x >= W) return;
+  for (int r = threadIdx.y; r < MP_TILE && y0 + r < H; r += MP_ROWS) {
+    const long p = (f * HW + (long)(y0 + r) * W + x) * 3;
+    uint8_t rgb[3] = {frames[p], frames[p + 1], frames[p + 2]};
+    const int* c = s_lab + (r + 3) * MP_LD + threadIdx.x + 3;
+    int w[49];                                     // the window in registers (only the reached entries are read)
+#pragma unroll
+    for (int i = 0; i < 49; ++i) w[i] = c[(i / 7 - 3) * MP_LD + i % 7 - 3];
+    pp_paint_pixel(w + 24, 7, s_max, s_pal, n_colors, alpha, oma, rgb);
+    out[p] = rgb[0];
+    out[p + 1] = rgb[1];
+    out[p + 2] = rgb[2];
+  }
+}
+
+extern "C" size_t pp_mask_paint_workspace_bytes(int T, int H, int W) {
+  if (T < 1 || H < 1 || W < 1) return 0;
+  return (size_t)T * 256 * sizeof(float) + (size_t)T * mp_tiles(H, W) * MP_CANDS * sizeof(float);
+}
+
+extern "C" int pp_mask_paint_u8(const uint8_t* frames, const uint8_t* labels, const uint8_t* palette, int n_colors,
+                                const double* alpha, uint8_t* out, int T, int H, int W, void* workspace, size_t workspace_bytes,
+                                cudaStream_t stream) {
+  if (T < 1 || T > 65535 || H < 1 || W < 1 || n_colors < 2 || alpha == nullptr) return PP_ERR_SHAPE;
+  const long ntiles = mp_tiles(H, W);
+  if (ntiles > INT_MAX) return PP_ERR_SHAPE;
+  if (workspace == nullptr || workspace_bytes < pp_mask_paint_workspace_bytes(T, H, W)) return PP_ERR_WORKSPACE;
+  if ((uintptr_t)workspace & 3) return PP_ERR_ALIGN;
+  float* maxima = static_cast<float*>(workspace);
+  float* partial = maxima + (size_t)T * 256;
+  const int tiles_x = (W + MP_TILE - 1) / MP_TILE;
+  const dim3 block(MP_TILE, MP_ROWS), grid((unsigned)ntiles, T);
+  k_mask_paint_partial<<<grid, block, 0, stream>>>(labels, H, W, tiles_x, ntiles, partial);
+  PP_LAUNCH_CHECK();
+  k_mask_paint_maxima<<<T, block, 0, stream>>>(labels, H, W, ntiles, partial, maxima);
+  PP_LAUNCH_CHECK();
+  k_mask_paint_u8<<<grid, block, 0, stream>>>(frames, labels, palette, n_colors < 257 ? n_colors : 257, alpha[0], alpha[1],
+                                              maxima, out, H, W, tiles_x);
   PP_LAUNCH_CHECK();
   return PP_OK;
 }

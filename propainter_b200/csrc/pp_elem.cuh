@@ -578,6 +578,88 @@ PP_HD void pp_flowviz_pt(float u, float v, float den, int bgr, uint8_t* rgb) {
   }
 }
 
+// ---- tracking preview: BaseTracker.track's painter loop (web-demos/hugging_face/tracker/base_tracker.py:90-95) ----
+// mask_painter (tools/painter.py:137-157) at contour_width 3 paints object k over the image in two steps: the fill where
+// the label is k, then the contour colour where |clip(fore - back, -3, 3)| / max over the frame, with values above 0.5 set
+// to 1, has 1 - that value > 0.5 (vis_add_mask, :106-110).  fore / back are cv2.distanceTransform(DIST_L2, 3) of the
+// object and of its complement: a 3x3 chamfer accumulated in float32 with steps a = 0.955 (axial), b = 1.3693 (diagonal).
+// Clipped at 3, only six path sums stay below 3, so min(DT, 3) of a pixel is the least of the table below over the
+// opposite-class pixels of its 7x7 window (pixels outside the frame never count), or 3 if there are none.
+
+// path sum of the chamfer to offset (dy, dx), in cv2's float32 order; 3 (the clip) for every longer path and for (0, 0)
+PP_HD float pp_paint_chamfer(int dy, int dx) {
+  dy = dy < 0 ? -dy : dy;
+  dx = dx < 0 ? -dx : dx;
+  const int p = dy > dx ? dy : dx, q = dy > dx ? dx : dy;
+  const float a = 0.955f, b = 1.3693f;
+  if (p == 1) return q == 0 ? a : b;
+  if (p == 2) return q == 0 ? PP_ADD(a, a) : (q == 1 ? PP_ADD(a, b) : PP_ADD(b, b));
+  if (p == 3 && q == 0) return PP_ADD(PP_ADD(a, a), a);
+  return 3.0f;
+}
+// v = |clip(fore - back, -3, 3)| of the pixel at c for object k: min(DT, 3) inside the object against the pixels that are
+// not k, outside it against the pixels that are.  c points into a label window (rows ld apart, -1 outside the frame)
+// holding the 3 rows / columns around it.
+template <typename L>
+PP_HD float pp_paint_dist(const L* c, int ld, int k) {
+  const bool in = c[0] == k;
+  float v = 3.0f;
+#pragma unroll
+  for (int dy = -3; dy <= 3; ++dy)
+#pragma unroll
+    for (int dx = -3; dx <= 3; ++dx) {
+      const float d = pp_paint_chamfer(dy, dx);
+      const int l = c[dy * ld + dx];
+      if (d < 3.0f && l >= 0 && (l == k) != in) v = fminf(v, d);
+    }
+  return v;
+}
+// the smallest non-zero id above prev among the pixel and the window pixels the table reaches (256 if none).  An id
+// that only occurs farther away has v = 3 here and paints nothing at this pixel.
+template <typename L>
+PP_HD int pp_paint_next_id(const L* c, int ld, int prev) {
+  int k = 256;
+#pragma unroll
+  for (int dy = -3; dy <= 3; ++dy)
+#pragma unroll
+    for (int dx = -3; dx <= 3; ++dx) {
+      const int l = c[dy * ld + dx];
+      if ((pp_paint_chamfer(dy, dx) < 3.0f || (dy == 0 && dx == 0)) && l > prev && l < k) k = l;
+    }
+  return k;
+}
+// The contour test 1 - v / M > 0.5 with M the maximum of v over the frame (> 0: every pixel has v >= a), in the
+// reference's two float32 roundings: it differs from v / M < 0.5 where v / M lies within an ulp of 0.5 (v = b, M = 2b).
+PP_HD bool pp_paint_contour(float v, float M) { return PP_SUB(1.0f, PP_DIV(v, M)) > 0.5f; }
+// the fill of one channel in float64 as numpy evaluates it: img * (1 - alpha) + color * alpha, truncated to uint8;
+// oma = 1 - alpha as the caller computed it (0.30000000000000004 for alpha = 0.7)
+PP_HD uint8_t pp_paint_fill(uint8_t img, uint8_t color, double alpha, double oma) {
+  return (uint8_t)(int)PP_DADD(PP_DMUL((double)img, oma), PP_DMUL((double)color, alpha));
+}
+// The ids of a frame whose maximum M can be below 3: M < 3 needs v < 3 at every pixel, pixel (0, 0) included, so they
+// are among the ids k with v < 3 at (0, 0) (at most 11 ids reach a corner).  c is (0, 0)'s window; out[] gets them in
+// ascending order; returns their count.  Every other present id has M = 3.
+template <typename L>
+PP_HD int pp_paint_candidates(const L* c, int ld, int* out) {
+  int n = 0;
+  for (int k = pp_paint_next_id(c, ld, 0); k < 256; k = pp_paint_next_id(c, ld, k))
+    if (pp_paint_dist(c, ld, k) < 3.0f) out[n++] = k;
+  return n;
+}
+// One pixel rgb of the loop: each id k of its window in ascending order (the reference skips absent ids; ids of the
+// window are present), fill with palette row k + 1 where the pixel is k, then the contour with row 1 where it lies on
+// k's contour.  maxima[k]: M of id k in this frame.  Ids with no palette row (k + 1 >= n_colors) are not painted.
+template <typename L>
+PP_HD void pp_paint_pixel(const L* c, int ld, const float* maxima, const uint8_t* palette, int n_colors, double alpha,
+                          double oma, uint8_t* rgb) {
+  for (int k = pp_paint_next_id(c, ld, 0); k < 256 && k + 1 < n_colors; k = pp_paint_next_id(c, ld, k)) {
+    if (c[0] == k)
+      for (int ch = 0; ch < 3; ++ch) rgb[ch] = pp_paint_fill(rgb[ch], palette[(k + 1) * 3 + ch], alpha, oma);
+    if (pp_paint_contour(pp_paint_dist(c, ld, k), maxima[k]))
+      for (int ch = 0; ch < 3; ++ch) rgb[ch] = palette[3 + ch];
+  }
+}
+
 // ---- I3D (core/metrics.py:195-569) ----
 // TF 'same' padding of a k-tap, stride-s window over n samples: Unit3D.compute_pad / MaxPool3dSamePadding.compute_pad
 // (core/metrics.py:196-200,258-262).  The front takes pad / 2, the back the rest, so even pads of 5 split 2 / 3.

@@ -9,6 +9,7 @@ copy of the raw frames / masks and one device -> host copy of the result.
 
 ``track`` is the demo's Cutie stage (web-demos/hugging_face/track_anything.py:21-36, app.py:264-290): label masks for
 every frame from the first frame's template, on the device, ready for ``inpaint``.  The tracker is built on first use.
+``track(..., return_painted=True)`` and ``paint_masks`` give the demo's painted previews (ops.mask_paint_u8).
 """
 import numpy as np
 import torch
@@ -68,10 +69,12 @@ class ProInpainter:
         return list(comp.cpu().numpy())
 
     @torch.no_grad()
-    def track(self, npframes, template_mask, return_probs=False):
+    def track(self, npframes, template_mask, return_probs=False, return_painted=False, palette=None):
         """The demo's tracking stage: frames T x [H,W,3] uint8 and the first frame's label mask [H,W] (object ids, 0 =
-        background) -> uint8 label masks [T,H,W] on the device (plus probabilities [T,objects+1,H,W] if return_probs).
-        Zeroing the objects that should not be removed before ``inpaint`` is the caller's step, as in the demo."""
+        background) -> uint8 label masks [T,H,W] on the device (plus probabilities [T,objects+1,H,W] if return_probs,
+        and, last, the painted preview frames uint8 [T,H,W,3] the demo shows after tracking if return_painted; see
+        MaskTracker.track).  Zeroing the objects that should not be removed before ``inpaint`` is the caller's step, as in
+        the demo."""
         if self.tracker is None:
             from .model.cutie import CUTIE
             from .tracker import MaskTracker
@@ -79,4 +82,25 @@ class ProInpainter:
             if self.cutie_checkpoint is not None:
                 net.load_weights(torch.load(self.cutie_checkpoint, map_location="cpu"))
             self.tracker = MaskTracker(net, self.device)
-        return self.tracker.track(npframes, template_mask, return_probs=return_probs)
+        return self.tracker.track(npframes, template_mask, return_probs=return_probs, return_painted=return_painted,
+                                  palette=palette)
+
+    @torch.no_grad()
+    def paint_masks(self, frames, masks, palette=None):
+        """The template preview of the demo's show_mask (app.py:191-197): frames uint8 [H,W,3] (or a clip [T,H,W,3]) and
+        the demo's mask list, mask i (0/1 or non-zero = object, shaped like frames[..., 0]) painted as object i + 1 with
+        palette row i + 2 -> uint8 like frames, on the device.  Pass all-zero masks for the entries not selected.  It is
+        show_mask's painting when the masks do not overlap; where they do, the later mask's id takes the pixel."""
+        fr = frames if torch.is_tensor(frames) else torch.from_numpy(np.ascontiguousarray(frames, dtype=np.uint8))
+        fr = fr.to(self.device).contiguous()
+        single = fr.dim() == 3
+        if len(masks) > 255:
+            raise ValueError(f"paint_masks: at most 255 masks, got {len(masks)}")
+        labels = torch.zeros(fr.shape[:-1], dtype=torch.uint8, device=self.device)
+        for i, m in enumerate(masks):
+            m = (m if torch.is_tensor(m) else torch.from_numpy(np.asarray(m))).to(self.device)
+            if tuple(m.shape) != tuple(labels.shape):
+                raise ValueError(f"paint_masks: mask {i} {tuple(m.shape)} does not match the frames {tuple(labels.shape)}")
+            labels[m != 0] = i + 1
+        out = ops.mask_paint_u8(fr[None] if single else fr, labels[None] if single else labels, palette)
+        return out[0] if single else out

@@ -7,6 +7,7 @@ import collections
 import ctypes
 import math
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -1145,4 +1146,75 @@ def cutie_labels(prob, lut, H, W, out=None):
     check(_lib.lib().pp_cutie_labels(_p(_dense(prob)), K, _p(_dense(lut), torch.uint8), _p(_dense(out), torch.uint8), H, W,
                                      _stream()), "pp_cutie_labels")
     _count(1)
+    return out
+
+
+# ---------------------------------------------------------------- tracking preview (tools/painter.py mask_painter)
+def paint_palette():
+    """The package's default palette for mask_paint_u8: uint8 [257,3], so every uint8 id k has its row k + 1.  Row 0 is
+    black and row 1 white (the contour colour, as in the web demo); row k >= 2 is colour k - 1 of the PASCAL VOC label
+    colormap (the bits of k - 1 spread over R, G, B from the most significant bit down), so object 1 is (128, 0, 0),
+    object 2 (0, 128, 0), object 3 (128, 128, 0).  The demo's own 22-colour table is passed as `palette` where its exact
+    colours are wanted."""
+    pal = np.zeros((257, 3), np.uint8)
+    pal[1] = 255
+    for i in range(1, 256):
+        c, rgb = i, [0, 0, 0]
+        for j in range(8):
+            for ch in range(3):
+                rgb[ch] |= ((c >> ch) & 1) << (7 - j)
+            c >>= 3
+        pal[i + 1] = rgb
+    return pal
+
+
+_PAINT_PALETTE = {}                                # device -> paint_palette() there, made on first use
+
+
+def mask_paint_u8(frames_u8, labels_u8, palette=None, mask_alpha=0.7, out=None):
+    """The web demo's tracking preview (BaseTracker.track's painter loop, base_tracker.py:90-95) for a whole clip on the
+    device: frames uint8 [T,H,W,3] and label masks uint8 [T,H,W] (0 = background) -> painted uint8 [T,H,W,3].  Each id k
+    present in a frame, in ascending order, is filled with palette row k + 1 at mask_alpha and outlined with row 1
+    (mask_painter, tools/painter.py:137-157, contour width 3); bytes equal the reference's for the same palette.
+    palette: uint8 [N,3] (tensor or array), default paint_palette().  `out` may be frames_u8 itself.  ValueError for CPU
+    tensors, other dtypes or shapes, a palette that is not uint8 [N,3] with N >= 2, mask_alpha outside [0, 1], and a
+    present id k with k + 1 >= N (where the reference raises IndexError)."""
+    for name, t in (("frames_u8", frames_u8), ("labels_u8", labels_u8)):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"mask_paint_u8: {name} must be a torch tensor, got {type(t).__name__}")
+    if frames_u8.dtype != torch.uint8 or frames_u8.dim() != 4 or frames_u8.shape[-1] != 3 or frames_u8.numel() == 0:
+        raise ValueError(f"mask_paint_u8: expected uint8 frames [T,H,W,3], got {frames_u8.dtype} {tuple(frames_u8.shape)}")
+    T, H, W, _ = frames_u8.shape
+    if labels_u8.dtype != torch.uint8 or tuple(labels_u8.shape) != (T, H, W):
+        raise ValueError(f"mask_paint_u8: expected uint8 labels [T,H,W] = {(T, H, W)}, got {labels_u8.dtype} "
+                         f"{tuple(labels_u8.shape)}")
+    pal = _PAINT_PALETTE.get(frames_u8.device) if palette is None else torch.as_tensor(palette)
+    if pal is None:
+        pal = torch.from_numpy(paint_palette())
+    if pal.dtype != torch.uint8 or pal.dim() != 2 or pal.shape[1] != 3 or pal.shape[0] < 2:
+        raise ValueError(f"mask_paint_u8: palette must be uint8 [N,3] with N >= 2, got {pal.dtype} {tuple(pal.shape)}")
+    alpha = float(mask_alpha)
+    if not 0.0 <= alpha <= 1.0:
+        raise ValueError(f"mask_paint_u8: mask_alpha must lie in [0, 1], got {mask_alpha}")
+    N = pal.shape[0]
+    if N < 257:
+        top = int(labels_u8.max())
+        if top + 1 >= N:
+            raise ValueError(f"mask_paint_u8: id {top} needs palette row {top + 1}, the palette has {N} rows")
+    if not frames_u8.is_cuda or labels_u8.device != frames_u8.device:
+        raise ValueError(f"mask_paint_u8: frames and labels must be on one CUDA device, got {frames_u8.device} / "
+                         f"{labels_u8.device} (there is no CPU path)")
+    pal = pal.to(frames_u8.device).contiguous()
+    if palette is None:
+        _PAINT_PALETTE[frames_u8.device] = pal
+    if out is None:
+        out = torch.empty_like(frames_u8)
+    elif not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.shape != frames_u8.shape or out.device != frames_u8.device:
+        raise ValueError("mask_paint_u8: out must be a uint8 tensor shaped and placed like frames_u8")
+    L = _lib.lib()
+    ws = torch.empty(L.pp_mask_paint_workspace_bytes(T, H, W), dtype=torch.uint8, device=frames_u8.device)
+    check(L.pp_mask_paint_u8(_p(_dense(frames_u8), torch.uint8), _p(_dense(labels_u8), torch.uint8), _p(pal, torch.uint8), N,
+                             (ctypes.c_double * 2)(alpha, 1.0 - alpha), _p(_dense(out), torch.uint8), T, H, W,
+                             _p(ws, torch.uint8), ws.numel(), _stream()), "pp_mask_paint_u8")
+    _count(3)
     return out

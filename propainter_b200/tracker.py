@@ -10,6 +10,8 @@ a top-k (30) readout.  What differs is where the work happens:
   * the memory read is one kernel (``ops.cutie_topk_readout``): no N x HW similarity, no dense affinity
   * frame conversion + padding + normalisation and argmax + unpad + id remapping are single kernels
     (``ops.cutie_frame_in`` / ``ops.cutie_labels``), so ``track`` returns the label masks on the device
+  * the painted preview frames (mask_painter per object, base_tracker.py:90-95) are one launch over the whole clip after
+    the loop (``ops.mask_paint_u8``), on request
 Long-term memory, flip augmentation, internal resizing and object chunking are not supported (ValueError).
 """
 import logging
@@ -271,10 +273,12 @@ class MaskTracker:
         return self.step_padded(frame_u8, mask_u8)[:, top:top + H, left:left + W]
 
     @torch.no_grad()
-    def track(self, frames_u8, template_mask_u8, return_probs=False):
+    def track(self, frames_u8, template_mask_u8, return_probs=False, return_painted=False, palette=None):
         """TrackingAnything.generator (track_anything.py:21-36) from a cleared memory: frames T x [H,W,3] uint8 (array,
         list or device tensor), the first frame's label mask [H,W] -> uint8 label masks [T,H,W] on the device, plus the
-        probabilities [T,objects+1,H,W] when return_probs."""
+        probabilities [T,objects+1,H,W] when return_probs.  return_painted: also the painted frames BaseTracker.track
+        returns (uint8 [T,H,W,3] on the device, ops.mask_paint_u8 with `palette` over the labels, one launch after the
+        loop), last: (labels, painted) or (labels, probs, painted)."""
         self.clear_memory()
         if torch.is_tensor(frames_u8):
             frames = frames_u8.to(self.device)
@@ -294,6 +298,7 @@ class MaskTracker:
             ops.cutie_labels(pred.contiguous(), self.out_lut, H, W, out=out[i])
             if return_probs:
                 probs.append(pred[:, top:top + H, left:left + W])
-        if return_probs:
-            return out, torch.stack(probs)
-        return out
+        res = (out, torch.stack(probs)) if return_probs else (out,)
+        if return_painted:
+            res += (ops.mask_paint_u8(frames.contiguous(), out, palette),)
+        return res if len(res) > 1 else out
