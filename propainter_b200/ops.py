@@ -28,6 +28,19 @@ def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def _launch(symbol, *args, launches=1):
+    """Call the library's `symbol` with args + the current stream, raise naming it if it fails, and count the
+    `launches` kernels it enqueues."""
+    global LAUNCHES
+    check(getattr(_lib.lib(), symbol)(*args, _stream()), symbol)
+    LAUNCHES += launches
+
+
+def _twin(symbol, t):
+    """(symbol, fp32) for the rows of tensor t, or (its fp16 twin symbol_f16, fp16) when t is fp16."""
+    return (symbol + "_f16", torch.float16) if t.dtype == torch.float16 else (symbol, torch.float32)
+
+
 def _p(t, dtype=torch.float32):
     if t is None:
         return None
@@ -38,10 +51,11 @@ def _p(t, dtype=torch.float32):
     return ctypes.c_void_p(t.data_ptr())
 
 
-def _dense(t):
-    if not t.is_contiguous():
+def _pd(t, dtype=torch.float32):
+    """_p of a tensor that must be contiguous."""
+    if t is not None and not t.is_contiguous():
         raise RuntimeError("tensor must be contiguous")
-    return t
+    return _p(t, dtype)
 
 
 def _pm(t, dtype=torch.float32):
@@ -76,30 +90,35 @@ def _level_array(levels):
 
 def corr_build(fmap, idx1, idx2, levels, h, w):
     """fmap [frames, h*w, D] pixel-major; idx1/idx2 int32 CUDA [n_pairs]; fills the 4 pyramid levels."""
-    L = _lib.lib()
     n_pairs = idx1.numel()
-    D = fmap.shape[-1]
-    check(L.pp_corr_build(_p(_dense(fmap)), D, _p(idx1, torch.int32), _p(idx2, torch.int32), n_pairs, _p(levels[0]), h, w,
-                          _stream()), "pp_corr_build")
-    check(L.pp_corr_pool_pyramid(_level_array(levels), n_pairs * h * w, h, w, _stream()), "pp_corr_pool_pyramid")
-    _count(4)
+    _launch("pp_corr_build", _pd(fmap), fmap.shape[-1], _p(idx1, torch.int32), _p(idx2, torch.int32), n_pairs, _p(levels[0]),
+            h, w)
+    _launch("pp_corr_pool_pyramid", _level_array(levels), n_pairs * h * w, h, w, launches=3)
 
 
 def corr_lookup(levels, coords, out=None, tma=True):
     """coords [B,h,w,2] -> [B,h,w,324].  tma=False selects the plain-load baseline kernel.  An fp16 `out` [B,h,w,ld >= 324]
     receives the taps rounded to nearest in channels [0, 324) of its rows."""
+    return _corr_lookup(levels, coords, None, out, tma)
+
+
+def corr_lookup_r(levels, coords, radius, out=None, tma=True):
+    """corr_lookup with window radius 3 (RAFT-small) or 4: coords [B,h,w,2] -> [B,h,w,4*(2*radius+1)**2]."""
+    return _corr_lookup(levels, coords, radius, out, tma)
+
+
+def _corr_lookup(levels, coords, radius, out, tma):
+    """radius None: corr_lookup's fixed-radius entries pp_corr_lookup[_ldg][_f16], else pp_corr_lookup[_ldg]_r."""
     B, h, w, _ = coords.shape
     if out is None:
-        out = torch.empty(B, h, w, 324, device=coords.device, dtype=torch.float32)
-    if out.dtype == torch.float16:
-        fn = _lib.lib().pp_corr_lookup_f16 if tma else _lib.lib().pp_corr_lookup_ldg_f16
-        check(fn(_level_array(levels), _p(_dense(coords)), _p(_dense(out), torch.float16), out.shape[-1], B, h, w, _stream()),
-              "pp_corr_lookup_f16")
-        _count(1)
-        return out
-    fn = _lib.lib().pp_corr_lookup if tma else _lib.lib().pp_corr_lookup_ldg
-    check(fn(_level_array(levels), _p(_dense(coords)), _p(_dense(out)), B, h, w, _stream()), "pp_corr_lookup")
-    _count(1)
+        out = torch.empty(B, h, w, 4 * (2 * (radius or 4) + 1) ** 2, device=coords.device, dtype=torch.float32)
+    sym = "pp_corr_lookup" if tma else "pp_corr_lookup_ldg"
+    if radius is None and out.dtype == torch.float16:
+        _launch(sym + "_f16", _level_array(levels), _pd(coords), _pd(out, torch.float16), out.shape[-1], B, h, w)
+    elif radius is None:
+        _launch(sym, _level_array(levels), _pd(coords), _pd(out), B, h, w)
+    else:
+        _launch(sym + "_r", _level_array(levels), radius, _pd(coords), _pd(out), B, h, w)
     return out
 
 
@@ -108,50 +127,32 @@ def corr_fmap_pyramid(fmap, h, w):
     [frames, (h>>l)*(w>>l), D]: the stored half of the on-the-fly correlation (AlternateCorrBlock)."""
     F_, _, D = fmap.shape
     pooled = [torch.empty(F_, (h >> l) * (w >> l), D, device=fmap.device, dtype=torch.float32) for l in (1, 2, 3)]
-    check(_lib.lib().pp_corr_fmap_pyramid(_p(_dense(fmap)), D, F_, h, w, (ctypes.c_void_p * 3)(*[p.data_ptr() for p in pooled]),
-                                          _stream()), "pp_corr_fmap_pyramid")
-    _count(3)
+    _launch("pp_corr_fmap_pyramid", _pd(fmap), D, F_, h, w, (ctypes.c_void_p * 3)(*[p.data_ptr() for p in pooled]), launches=3)
     return pooled
 
 
 def corr_lookup_otf(fmap, pooled, idx1, idx2, coords, out=None):
     """corr_lookup without the all-pairs volume: pair p correlates frame idx1[p] with idx2[p] (int32 CUDA [n_pairs]) of
     fmap [frames, h*w, 256] and its pooled levels (corr_fmap_pyramid) at lookup time.  coords [B,h,w,2] -> [B,h,w,324]."""
-    B, h, w, _ = coords.shape
-    if idx1.numel() != B or idx2.numel() != B:
-        raise RuntimeError("corr_lookup_otf: one (idx1, idx2) entry per coords batch row")
-    if out is None:
-        out = torch.empty(B, h, w, 324, device=coords.device, dtype=torch.float32)
-    levels = (ctypes.c_void_p * 3)(*[_p(_dense(p)).value for p in pooled])
-    check(_lib.lib().pp_corr_lookup_otf(_p(_dense(fmap)), levels, fmap.shape[-1], _p(idx1, torch.int32), _p(idx2, torch.int32), B,
-                                        _p(_dense(coords)), _p(_dense(out)), h, w, _stream()), "pp_corr_lookup_otf")
-    _count(1)
-    return out
-
-
-def corr_lookup_r(levels, coords, radius, out=None, tma=True):
-    """corr_lookup with window radius 3 (RAFT-small) or 4: coords [B,h,w,2] -> [B,h,w,4*(2*radius+1)**2]."""
-    B, h, w, _ = coords.shape
-    if out is None:
-        out = torch.empty(B, h, w, 4 * (2 * radius + 1) ** 2, device=coords.device, dtype=torch.float32)
-    fn = _lib.lib().pp_corr_lookup_r if tma else _lib.lib().pp_corr_lookup_ldg_r
-    check(fn(_level_array(levels), radius, _p(_dense(coords)), _p(_dense(out)), B, h, w, _stream()), "pp_corr_lookup_r")
-    _count(1)
-    return out
+    return _corr_lookup_otf(fmap, pooled, idx1, idx2, coords, None, out)
 
 
 def corr_lookup_otf_r(fmap, pooled, idx1, idx2, coords, radius, out=None):
     """corr_lookup_otf with (D, radius) = (256, 4) or (128, 3): fmap [frames, h*w, D] -> [B,h,w,4*(2*radius+1)**2]."""
+    return _corr_lookup_otf(fmap, pooled, idx1, idx2, coords, radius, out)
+
+
+def _corr_lookup_otf(fmap, pooled, idx1, idx2, coords, radius, out):
+    """radius None: pp_corr_lookup_otf (radius 4), else pp_corr_lookup_otf_r."""
+    sym, rad = ("pp_corr_lookup_otf", ()) if radius is None else ("pp_corr_lookup_otf_r", (radius,))
     B, h, w, _ = coords.shape
     if idx1.numel() != B or idx2.numel() != B:
-        raise RuntimeError("corr_lookup_otf_r: one (idx1, idx2) entry per coords batch row")
+        raise RuntimeError(f"{sym[3:]}: one (idx1, idx2) entry per coords batch row")
     if out is None:
-        out = torch.empty(B, h, w, 4 * (2 * radius + 1) ** 2, device=coords.device, dtype=torch.float32)
-    levels = (ctypes.c_void_p * 3)(*[_p(_dense(p)).value for p in pooled])
-    check(_lib.lib().pp_corr_lookup_otf_r(_p(_dense(fmap)), levels, fmap.shape[-1], radius, _p(idx1, torch.int32),
-                                          _p(idx2, torch.int32), B, _p(_dense(coords)), _p(_dense(out)), h, w, _stream()),
-          "pp_corr_lookup_otf_r")
-    _count(1)
+        out = torch.empty(B, h, w, 4 * (2 * (radius or 4) + 1) ** 2, device=coords.device, dtype=torch.float32)
+    levels = (ctypes.c_void_p * 3)(*[_pd(p).value for p in pooled])
+    _launch(sym, _pd(fmap), levels, fmap.shape[-1], *rad, _p(idx1, torch.int32), _p(idx2, torch.int32), B, _pd(coords), _pd(out),
+            h, w)
     return out
 
 
@@ -160,8 +161,7 @@ def upflow8(flow_lr):
     with 8 * F.interpolate(flow, (8h, 8w), mode="bilinear", align_corners=True) on the CPU."""
     n, h, w, _ = flow_lr.shape
     out = torch.empty(n, 2, 8 * h, 8 * w, device=flow_lr.device, dtype=torch.float32)
-    check(_lib.lib().pp_upflow8(_p(_dense(flow_lr)), _p(out), n, h, w, _stream()), "pp_upflow8")
-    _count(1)
+    _launch("pp_upflow8", _pd(flow_lr), _p(out), n, h, w)
     return out
 
 
@@ -170,22 +170,18 @@ def convex_upsample(mask_pm, flow_lr, mask_scale=0.25):
     n, h, w, _ = flow_lr.shape
     mp, ld = _pm(mask_pm)
     out = torch.empty(n, 2, 8 * h, 8 * w, device=flow_lr.device, dtype=torch.float32)
-    check(_lib.lib().pp_convex_upsample(mp, ld, mask_scale, _p(_dense(flow_lr)), _p(out), n, h, w, _stream()),
-          "pp_convex_upsample")
-    _count(1)
+    _launch("pp_convex_upsample", mp, ld, mask_scale, _pd(flow_lr), _p(out), n, h, w)
     return out
 
 
 def img_prop_scan(frames, flows_f, flows_b, masks, nearest=True):
     """frames [t,3,H,W], flows [t-1,2,H,W], masks [t,1,H,W] (planar) -> (frames_out, masks_out)."""
-    L = _lib.lib()
     t, _, H, W = frames.shape
-    ws_bytes = L.pp_img_prop_scan_workspace_bytes(t, H, W)
+    ws_bytes = _lib.lib().pp_img_prop_scan_workspace_bytes(t, H, W)
     ws = torch.empty(ws_bytes // 4, device=frames.device, dtype=torch.float32)
     of, om = torch.empty_like(frames), torch.empty_like(masks)
-    check(L.pp_img_prop_scan(_p(_dense(frames)), _p(_dense(flows_f)), _p(_dense(flows_b)), _p(_dense(masks)), _p(of),
-                             _p(om), _p(ws), ws_bytes, t, H, W, int(bool(nearest)), _stream()), "pp_img_prop_scan")
-    _count(2 * (t - 1))
+    _launch("pp_img_prop_scan", _pd(frames), _pd(flows_f), _pd(flows_b), _pd(masks), _p(of), _p(om), _p(ws), ws_bytes, t, H, W,
+            int(bool(nearest)), launches=2 * (t - 1))
     return of, om
 
 
@@ -193,19 +189,17 @@ def img_prop_scan_u8h(frames_u8, masks, flows_f, flows_b, out_frames, out_masks,
     """img_prop_scan on half-precision clip storage, composited: frames_u8 uint8 [t,H,W,3], masks float {0,1} [t,1,H,W],
     fp16 flows [t-1,2,H,W].  Writes frames [lo, hi) of frames * (1 - masks) + prop * masks into fp16 out_frames
     [hi-lo,3,H,W] and of the updated masks into fp16 out_masks [hi-lo,1,H,W] (views of clip buffers); the scan is fp32."""
-    L = _lib.lib()
     t, H, W, _ = frames_u8.shape
     hi = t if hi is None else hi
     if tuple(out_frames.shape) != (hi - lo, 3, H, W) or tuple(out_masks.shape) != (hi - lo, 1, H, W):
         raise RuntimeError(f"img_prop_scan_u8h: outputs for frames [{lo}, {hi}) of a {H}x{W} clip, got "
                            f"{tuple(out_frames.shape)} / {tuple(out_masks.shape)}")
-    ws_bytes = L.pp_img_prop_scan_u8h_workspace_bytes(t, H, W)
+    ws_bytes = _lib.lib().pp_img_prop_scan_u8h_workspace_bytes(t, H, W)
     ws = torch.empty(ws_bytes // 4, device=frames_u8.device, dtype=torch.float32)
     f16 = torch.float16
-    check(L.pp_img_prop_scan_u8h(_p(_dense(frames_u8), torch.uint8), _p(_dense(masks)), _p(_dense(flows_f), f16),
-                                 _p(_dense(flows_b), f16), _p(_dense(out_frames), f16), _p(_dense(out_masks), f16), _p(ws),
-                                 ws_bytes, t, H, W, lo, hi, int(bool(nearest)), _stream()), "pp_img_prop_scan_u8h")
-    _count(t + hi - (lo > 0) if hi > lo else 0)
+    _launch("pp_img_prop_scan_u8h", _pd(frames_u8, torch.uint8), _pd(masks), _pd(flows_f, f16), _pd(flows_b, f16),
+            _pd(out_frames, f16), _pd(out_masks, f16), _p(ws), ws_bytes, t, H, W, lo, hi, int(bool(nearest)),
+            launches=t + hi - (lo > 0) if hi > lo else 0)
     return out_frames, out_masks
 
 
@@ -216,9 +210,7 @@ def prop_cond(cur, prop, fprop, fcheck, mcur, cond, bb, first):
     pp_, ldp = _pm(prop) if prop is not None else (None, ldc)
     cdp, ldcd = _pm(cond) if cond is not None else (None, 2 * C + 8)
     bp, ldb = _pm(bb)
-    check(_lib.lib().pp_prop_cond(cp, ldc, pp_, ldp, _p(fprop), _p(fcheck), _p(_dense(mcur)), cdp, ldcd, bp, ldb, h, w,
-                                  C, int(bool(first)), _stream()), "pp_prop_cond")
-    _count(1)
+    _launch("pp_prop_cond", cp, ldc, pp_, ldp, _p(fprop), _p(fcheck), _pd(mcur), cdp, ldcd, bp, ldb, h, w, C, int(bool(first)))
 
 
 def deform_align(x, o, flow, max_res, w_packed, bias, out, o_bias=None):
@@ -229,12 +221,10 @@ def deform_align(x, o, flow, max_res, w_packed, bias, out, o_bias=None):
     xp, ldx = _pm(x)
     op, ldo = _pm(o)
     outp, ldout = _pm(out)
-    L = _lib.lib()
-    ws_bytes = L.pp_deform_align_workspace_bytes(H, W)
+    ws_bytes = _lib.lib().pp_deform_align_workspace_bytes(H, W)
     ws = torch.empty(max(ws_bytes // 4, 4), device=x.device, dtype=torch.float32)
-    check(L.pp_deform_align(xp, ldx, op, ldo, _p(o_bias), _p(flow), float(max_res), _p(_dense(w_packed)), _p(bias), outp, ldout,
-                            H, W, Cin, out.shape[-1], _p(ws), ws_bytes, _stream()), "pp_deform_align")
-    _count(3)                                                    # tap pre-pass, GEMM, (split-K reduce)
+    _launch("pp_deform_align", xp, ldx, op, ldo, _p(o_bias), _p(flow), float(max_res), _pd(w_packed), _p(bias), outp, ldout, H, W,
+            Cin, out.shape[-1], _p(ws), ws_bytes, launches=3)       # tap pre-pass, GEMM, (split-K reduce)
     return out
 
 
@@ -302,7 +292,7 @@ def _conv_params(segs, KH, KW, Cout, w_packed=None, bias=None, act="none", slope
     if w_packed is not None and tuple(w_packed.shape) != (Cout, kblocks * KH * KW * cb):
         raise RuntimeError(f"conv_umma: packed weight {tuple(w_packed.shape)} does not match {(Cout, kblocks * KH * KW * cb)}")
     prm.n, prm.H, prm.W, prm.KH, prm.KW = n, H, W, KH, KW
-    prm.w_packed, prm.Cout = _p(_dense(w_packed), dt).value if w_packed is not None else None, Cout
+    prm.w_packed, prm.Cout = _pd(w_packed, dt).value if w_packed is not None else None, Cout
     prm.bias = _p(bias).value if bias is not None else None
     for name, t in (("pre", pre), ("res", res), ("out", out)):
         if t is None:
@@ -325,11 +315,9 @@ def conv_umma(segs, w_packed, KH, KW, Cout, bias=None, act="none", slope=0.0, pr
     views = the channel-concatenated input; w_packed from pack_conv_weight(weight, [C_i...]); pre / res / out
     [n,H,W,Cout] views (channel slices of wider buffers allowed).  Returns out."""
     if out is None and segs:
-        n, H, W, _ = segs[0].shape
-        out = torch.empty(n, H, W, Cout, device=segs[0].device, dtype=torch.float32)
+        out = segs[0].new_empty(*segs[0].shape[:3], Cout)
     prm = _conv_params(segs, KH, KW, Cout, w_packed, bias, act, slope, pre, res, post_relu, out, round_tf32, bn, tile_w, tile_m)
-    check(_lib.lib().pp_conv2d_umma(ctypes.byref(prm), _stream()), "pp_conv2d_umma")
-    _count(1)
+    _launch("pp_conv2d_umma", ctypes.byref(prm))
     return out
 
 
@@ -339,16 +327,14 @@ def conv_umma_f16(segs, w_packed, KH, KW, Cout, bias=None, act="none", slope=0.0
     bias / pre / res fp32, fp32 accumulation and epilogue.  Writes the fp32 `out` and / or the fp16 `out16` (rounded to
     nearest once; both from one pass when both are given; neither: a new out16).  Returns out16, else out."""
     if out is None and out16 is None:
-        n, H, W, _ = segs[0].shape
-        out16 = torch.empty(n, H, W, Cout, device=segs[0].device, dtype=torch.float16)
+        out16 = segs[0].new_empty(*segs[0].shape[:3], Cout)
     prm = _conv_params(segs, KH, KW, Cout, w_packed, bias, act, slope, pre, res, post_relu, out, False, bn, tile_w, tile_m, half=True)
     p16, ld16 = (None, 0)
     if out16 is not None:
         if tuple(out16.shape) != (prm.n, prm.H, prm.W, Cout):
             raise RuntimeError(f"conv_umma_f16: out16 shape {tuple(out16.shape)} != {(prm.n, prm.H, prm.W, Cout)}")
         p16, ld16 = _pm4(out16, torch.float16)
-    check(_lib.lib().pp_conv2d_umma_f16(ctypes.byref(prm), p16, ld16, _stream()), "pp_conv2d_umma_f16")
-    _count(1)
+    _launch("pp_conv2d_umma_f16", ctypes.byref(prm), p16, ld16)
     return out16 if out16 is not None else out
 
 
@@ -361,8 +347,8 @@ def conv_plan(segs, KH, KW, Cout, bn=0, tile_w=0, tile_m=0, out=None, pre=None, 
     (n, H, W, C_i).  Raises where conv_umma would refuse the plan."""
     prm = _conv_params(segs, KH, KW, Cout, bias=bias, pre=pre, res=res, out=out, bn=bn, tile_w=tile_w, tile_m=tile_m, half=half)
     vals = [ctypes.c_int(0) for _ in range(5)]
-    fn = _lib.lib().pp_conv2d_umma_plan_f16 if half else _lib.lib().pp_conv2d_umma_plan
-    check(fn(ctypes.byref(prm), *[ctypes.byref(v) for v in vals]), "pp_conv2d_umma_plan")
+    sym = "pp_conv2d_umma_plan_f16" if half else "pp_conv2d_umma_plan"
+    check(getattr(_lib.lib(), sym)(ctypes.byref(prm), *[ctypes.byref(v) for v in vals]), sym)
     return ConvPlan(*[v.value for v in vals])
 
 
@@ -381,10 +367,8 @@ def deform_gather(x, o, flow, max_res, cols=None, o_bias=None, x2=None):
     op, ldo = _pm4(o)
     if cols is None:
         cols = torch.empty(n, H, W, 9 * Cin, device=x.device, dtype=torch.float32)
-    fn = _lib.lib().pp_deform_gather_f16 if cols.dtype == torch.float16 else _lib.lib().pp_deform_gather
-    check(fn(xp, ldx, x2p, ldx2, op, ldo, _p(o_bias), _p(_dense(flow)) if flow is not None else None, float(max_res),
-             _p(_dense(cols), cols.dtype), n, H, W, Cin, _stream()), "pp_deform_gather")
-    _count(1)
+    sym, dt = _twin("pp_deform_gather", cols)
+    _launch(sym, xp, ldx, x2p, ldx2, op, ldo, _p(o_bias), _pd(flow), float(max_res), _pd(cols, dt), n, H, W, Cin)
     return cols
 
 
@@ -407,14 +391,11 @@ def flow_warp_fbcheck(feat, fprop, fcheck=None, warped=None, aux=None, want_warp
         if aux is None:
             aux = torch.empty(n, h, w, 4, device=fprop.device, dtype=torch.float32)
         ap, lda = _pm4(aux)
-    fc = _p(_dense(fcheck)) if fcheck is not None else None
+    args = (fp_, ldf, _pd(fprop), _pd(fcheck), wp_, ldw, ap, lda, n, h, w, C)
     if f16:
-        check(_lib.lib().pp_flow_warp_fbcheck_f16(fp_, ldf, _p(_dense(fprop)), fc, wp_, ldw, ap, lda, n, h, w, C, _stream()),
-              "pp_flow_warp_fbcheck_f16")
+        _launch("pp_flow_warp_fbcheck_f16", *args)
     else:
-        check(_lib.lib().pp_flow_warp_fbcheck(fp_, ldf, _p(_dense(fprop)), fc, wp_, ldw, ap, lda, n, h, w, C, int(bool(round_tf32)),
-                                              _stream()), "pp_flow_warp_fbcheck")
-    _count(1)
+        _launch("pp_flow_warp_fbcheck", *args, int(bool(round_tf32)))
     return warped, aux
 
 
@@ -444,22 +425,15 @@ def gen_prep(flows_f, flows_b, masks_in, masks_upd, lt):
     dsf = torch.empty(max(lt - 1, 1), h, w, 2, device=dev, dtype=torch.float32)
     dsb = torch.empty_like(dsf)
     pmask = torch.empty(lt, h, w, 2, device=dev, dtype=torch.float32)
-    if flows_f.dtype == torch.float16:                         # half-precision clip storage, widened in the kernel
-        check(_lib.lib().pp_gen_prep_f16(_p(_dense(flows_f), torch.float16), _p(_dense(flows_b), torch.float16), _p(_dense(masks_in)),
-                                         _p(_dense(masks_upd)), _p(dsf), _p(dsb), _p(pmask), lt, H, W, _stream()), "pp_gen_prep_f16")
-    else:
-        check(_lib.lib().pp_gen_prep(_p(_dense(flows_f)), _p(_dense(flows_b)), _p(_dense(masks_in)), _p(_dense(masks_upd)),
-                                     _p(dsf), _p(dsb), _p(pmask), lt, H, W, _stream()), "pp_gen_prep")
-    _count(1)
+    sym, dt = _twin("pp_gen_prep", flows_f)                     # fp16: half-precision clip storage, widened in the kernel
+    _launch(sym, _pd(flows_f, dt), _pd(flows_b, dt), _pd(masks_in), _pd(masks_upd), _p(dsf), _p(dsb), _p(pmask), lt, H, W)
     return dsf[:lt - 1], dsb[:lt - 1], pmask
 
 
 def window_mask(pmask, fh, fw, nwh, nww):
     lt, h, w, _ = pmask.shape
     flags = torch.empty(nwh * nww, device=pmask.device, dtype=torch.int32)
-    check(_lib.lib().pp_window_mask(_p(_dense(pmask)), lt, h, w, fh, fw, nwh, nww, _p(flags, torch.int32), _stream()),
-          "pp_window_mask")
-    _count(1)
+    _launch("pp_window_mask", _pd(pmask), lt, h, w, fh, fw, nwh, nww, _p(flags, torch.int32))
     return flags
 
 
@@ -480,32 +454,25 @@ def sparse_window_attn(qkv, pool_kv, key_tok, flags, t, NT, kf_start, kf_step, o
     if prm.nkf == 0:
         out.zero_()                 # empty key set: masked windows yield zeros (softmax over an empty dim), see the C entry
     prm.scale_log2 = LOG2E / math.sqrt(128.0)
-    for tns, tdt in ((qkv, dt), (pool_kv, dt), (out, dt), (key_tok, torch.int32), (flags, torch.int32)):
-        _p(_dense(tns) if tns is not out else tns, tdt)
+    for tns, tdt in ((qkv, dt), (pool_kv, dt), (key_tok, torch.int32), (flags, torch.int32)):
+        _pd(tns, tdt)                                           # the struct holds raw addresses: check what they point at
+    _p(out, dt)
     if dt == torch.float16:
-        fn, name = _lib.lib().pp_sparse_window_attn_f16, "pp_sparse_window_attn_f16"
+        sym = "pp_sparse_window_attn_f16"
     else:
-        fn, name = (_lib.lib().pp_sparse_window_attn if impl == "umma" else _lib.lib().pp_sparse_window_attn_mma), "pp_sparse_window_attn"
-    check(fn(ctypes.byref(prm), key_tok.shape[0], _stream()), name)
-    _count(2)
+        sym = "pp_sparse_window_attn" if impl == "umma" else "pp_sparse_window_attn_mma"
+    _launch(sym, ctypes.byref(prm), key_tok.shape[0], launches=2)
     return out
 
 
 def ffn_overlap_add(Y, frames, h, w, CH=40):
     """Y [frames*fh*fw, 49*CH] (tap-major columns) -> gelu(unfold(fold(Y)/norm)) same shape and dtype.  fp16 Y (the
     half-operand fc1 output): fp16 Z, summed in fp32 and rounded once."""
-    L = _lib.lib()
     Z = torch.empty_like(Y)
-    ws_bytes = L.pp_ffn_overlap_add_workspace_bytes(frames, h, w, CH)
+    ws_bytes = _lib.lib().pp_ffn_overlap_add_workspace_bytes(frames, h, w, CH)
     ws = torch.empty(ws_bytes // 4, device=Y.device, dtype=torch.float32)
-    if Y.dtype == torch.float16:
-        check(L.pp_ffn_overlap_add_f16(_p(_dense(Y), torch.float16), Y.shape[-1], _p(Z, torch.float16), Z.shape[-1], frames, h, w, CH,
-                                       _p(ws), ws_bytes, _stream()), "pp_ffn_overlap_add_f16")
-        _count(2)
-        return Z
-    check(L.pp_ffn_overlap_add(_p(_dense(Y)), Y.shape[-1], _p(Z), Z.shape[-1], frames, h, w, CH, _p(ws), ws_bytes,
-                               _stream()), "pp_ffn_overlap_add")
-    _count(2)
+    sym, dt = _twin("pp_ffn_overlap_add", Y)
+    _launch(sym, _pd(Y, dt), Y.shape[-1], _p(Z, dt), Z.shape[-1], frames, h, w, CH, _p(ws), ws_bytes, launches=2)
     return Z
 
 
@@ -514,16 +481,9 @@ def gru_gate(zr_pm, bias, net_view, z_out, rnet_view, pre=None):
     bias [2C] / pre [..,2C] optional addends.  fp16 zr_pm: rnet_view is fp16 too, net_view the fp32 state."""
     C = z_out.shape[-1]
     np_, ldn = _pm(net_view)
-    if zr_pm.dtype == torch.float16:
-        rp, ldr = _pm(rnet_view, torch.float16)
-        check(_lib.lib().pp_gru_gate_f16(_p(_dense(zr_pm), torch.float16), _p(bias), _p(_dense(pre)) if pre is not None else None, np_,
-                                         ldn, _p(_dense(z_out)), rp, ldr, z_out.numel() // C, C, _stream()), "pp_gru_gate_f16")
-        _count(1)
-        return
-    rp, ldr = _pm(rnet_view)
-    check(_lib.lib().pp_gru_gate(_p(_dense(zr_pm)), _p(bias), _p(_dense(pre)) if pre is not None else None, np_, ldn,
-                                 _p(_dense(z_out)), rp, ldr, z_out.numel() // C, C, _stream()), "pp_gru_gate")
-    _count(1)
+    sym, dt = _twin("pp_gru_gate", zr_pm)
+    rp, ldr = _pm(rnet_view, dt)
+    _launch(sym, _pd(zr_pm, dt), _p(bias), _pd(pre), np_, ldn, _pd(z_out), rp, ldr, z_out.numel() // C, C)
 
 
 def gru_update(q_pm, bias, z, net_view, net_copy=None, pre=None, h_img=None):
@@ -531,39 +491,25 @@ def gru_update(q_pm, bias, z, net_view, net_copy=None, pre=None, h_img=None):
     state net_view stays fp32, its fp16 image goes to h_img (a C-channel slice of the fp16 HX) and the fp16 net_copy."""
     C = z.shape[-1]
     np_, ldn = _pm(net_view)
-    if q_pm.dtype == torch.float16:
-        ip, ldi = _pm(h_img, torch.float16) if h_img is not None else (None, C)
-        check(_lib.lib().pp_gru_update_f16(_p(_dense(q_pm), torch.float16), _p(bias), _p(_dense(pre)) if pre is not None else None,
-                                           _p(_dense(z)), np_, ldn, ip, ldi,
-                                           _p(_dense(net_copy), torch.float16) if net_copy is not None else None, z.numel() // C, C,
-                                           _stream()), "pp_gru_update_f16")
-        _count(1)
-        return
-    if h_img is not None:
+    sym, dt = _twin("pp_gru_update", q_pm)
+    img = ()                                                    # pp_gru_update_f16's (h_img, ld)
+    if dt == torch.float16:
+        img = _pm(h_img, dt) if h_img is not None else (None, C)
+    elif h_img is not None:
         raise RuntimeError("gru_update: h_img is the fp16 image of the state (fp16 q_pm only)")
-    check(_lib.lib().pp_gru_update(_p(_dense(q_pm)), _p(bias), _p(_dense(pre)) if pre is not None else None, _p(_dense(z)), np_, ldn,
-                                   _p(_dense(net_copy)) if net_copy is not None else None, z.numel() // C, C, _stream()),
-          "pp_gru_update")
-    _count(1)
+    _launch(sym, _pd(q_pm, dt), _p(bias), _pd(pre), _pd(z), np_, ldn, *img, _pd(net_copy, dt), z.numel() // C, C)
 
 
 def raft_pack_motion(mot_pm, flow_pm, d0_view, d1_view, bias=None):
     """mot_pm [..,128] (channels 126,127 ignored), flow_pm [..,2] -> 128-channel slot views of HX and RX.
     With `bias`, mot_pm is the raw conv output and relu(mot + bias) is applied on the way.  fp16 mot_pm: fp16 HX / RX."""
-    dt = mot_pm.dtype
+    sym, dt = _twin("pp_raft_pack_motion", mot_pm)
     mp, ldm = _pm(mot_pm, dt)
     p0, ld0 = _pm(d0_view, dt)
     p1, ld1 = _pm(d1_view, dt)
     if ld0 != ld1:
         raise RuntimeError("HX / RX must share the pixel stride")
-    if dt == torch.float16:
-        check(_lib.lib().pp_raft_pack_motion_f16(mp, ldm, _p(bias), _p(_dense(flow_pm)), p0, p1, ld0, flow_pm.numel() // 2, _stream()),
-              "pp_raft_pack_motion_f16")
-        _count(1)
-        return
-    check(_lib.lib().pp_raft_pack_motion(mp, ldm, _p(bias), _p(_dense(flow_pm)), p0, p1, ld0, flow_pm.numel() // 2, _stream()),
-          "pp_raft_pack_motion")
-    _count(1)
+    _launch(sym, mp, ldm, _p(bias), _pd(flow_pm), p0, p1, ld0, flow_pm.numel() // 2)
 
 
 def raft_pack_motion_n(mot_pm, flow_pm, d0_view, d1_view, cmot, bias=None):
@@ -576,9 +522,7 @@ def raft_pack_motion_n(mot_pm, flow_pm, d0_view, d1_view, cmot, bias=None):
         raise RuntimeError("HX / RX must share the pixel stride")
     if mot_pm.shape[-1] < cmot or d0_view.shape[-1] < ((cmot + 5) & ~3) or (bias is not None and bias.numel() < cmot):
         raise RuntimeError("raft_pack_motion_n: channel counts too small for cmot")
-    check(_lib.lib().pp_raft_pack_motion_n(mp, ldm, _p(bias), _p(_dense(flow_pm)), p0, p1, ld0, flow_pm.numel() // 2, cmot,
-                                           _stream()), "pp_raft_pack_motion_n")
-    _count(1)
+    _launch("pp_raft_pack_motion_n", mp, ldm, _p(bias), _pd(flow_pm), p0, p1, ld0, flow_pm.numel() // 2, cmot)
 
 
 ACT = {"none": 0, "relu": 1, "leaky": 2, "sigmoid": 3, "tanh": 4}
@@ -593,39 +537,26 @@ def bias_act(x_pm, bias=None, act="none", slope=0.0, res=None, post_relu=False, 
     out = x_pm if out is None else out
     if out.shape != x_pm.shape or (res is not None and res.shape != x_pm.shape) or (pre is not None and pre.shape != x_pm.shape):
         raise RuntimeError("bias_act: shape mismatch")
-    if res is not None and res.dtype == torch.float16:
-        if x_pm.dtype != torch.float16 or out.dtype != torch.float16 or pre is not None:
+    f16, f32 = torch.float16, torch.float32
+    if res is not None and res.dtype == f16:
+        if x_pm.dtype != f16 or out.dtype != f16 or pre is not None:
             raise RuntimeError("bias_act: an fp16 residual needs fp16 x and out and no pre")
-        xp, ldx = _pm(x_pm, torch.float16)
-        op, ldo = _pm(out, torch.float16)
-        rp, ldr = _pm(res, torch.float16)
-        check(_lib.lib().pp_bias_act_f16_res(xp, ldx, _p(bias), rp, ldr, op, ldo, x_pm.numel() // C, C, ACT[act], float(slope),
-                                             int(bool(post_relu)), _stream()), "pp_bias_act_f16_res")
-        _count(1)
-        return out
-    if torch.float16 in (x_pm.dtype, out.dtype):
-        if not {x_pm.dtype, out.dtype} <= {torch.float16, torch.float32}:
+        sym, xdt, odt, rdt = "pp_bias_act_f16_res", f16, f16, f16
+    elif f16 in (x_pm.dtype, out.dtype):
+        if not {x_pm.dtype, out.dtype} <= {f16, f32}:
             raise RuntimeError(f"bias_act: x / out must be fp32 or fp16, got {x_pm.dtype} / {out.dtype}")
-        xp, ldx = _pm(x_pm, x_pm.dtype)
-        op, ldo = _pm(out, out.dtype)
-        rp, ldr = _pm(res) if res is not None else (None, C)
-        pp, ldp = _pm(pre) if pre is not None else (None, C)
-        check(_lib.lib().pp_bias_act_f16(xp, ldx, int(x_pm.dtype == torch.float16), _p(bias), pp, ldp, rp, ldr, op, ldo,
-                                         int(out.dtype == torch.float16), x_pm.numel() // C, C, ACT[act], float(slope),
-                                         int(bool(post_relu)), _stream()), "pp_bias_act_f16")
-        _count(1)
-        return out
-    xp, ldx = _pm(x_pm)
-    op, ldo = _pm(out)
-    rp, ldr = _pm(res) if res is not None else (None, C)
-    if pre is not None:
-        pp, ldp = _pm(pre)
-        check(_lib.lib().pp_bias_act_pre(xp, ldx, _p(bias), pp, ldp, rp, ldr, op, ldo, x_pm.numel() // C, C, ACT[act], float(slope),
-                                         int(bool(post_relu)), _stream()), "pp_bias_act_pre")
+        sym, xdt, odt, rdt = "pp_bias_act_f16", x_pm.dtype, out.dtype, f32
     else:
-        check(_lib.lib().pp_bias_act(xp, ldx, _p(bias), rp, ldr, op, ldo, x_pm.numel() // C, C, ACT[act], float(slope),
-                                     int(bool(post_relu)), _stream()), "pp_bias_act")
-    _count(1)
+        sym, xdt, odt, rdt = "pp_bias_act" if pre is None else "pp_bias_act_pre", f32, f32, f32
+    xp, ldx = _pm(x_pm, xdt)
+    op, ldo = _pm(out, odt)
+    rp, ldr = _pm(res, rdt) if res is not None else (None, C)
+    tail = (x_pm.numel() // C, C, ACT[act], float(slope), int(bool(post_relu)))
+    if sym == "pp_bias_act_f16":                                # takes the row types, and pre always
+        pp, ldp = _pm(pre) if pre is not None else (None, C)
+        _launch(sym, xp, ldx, int(xdt == f16), _p(bias), pp, ldp, rp, ldr, op, ldo, int(odt == f16), *tail)
+    else:
+        _launch(sym, xp, ldx, _p(bias), *(_pm(pre) if pre is not None else ()), rp, ldr, op, ldo, *tail)
     return out
 
 
@@ -645,9 +576,7 @@ def sc_fold(cols, bmap, frames, h, w, out=None):
     out = torch.empty(frames, h, w, C, device=cols.device, dtype=torch.float16) if out is None else out
     if tuple(out.shape) != (frames, h, w, C):
         raise RuntimeError("sc_fold: out shape mismatch")
-    check(_lib.lib().pp_sc_fold_f16(_p(cols, torch.float16), cols.stride(0), _p(_dense(bmap)), _p(_dense(out), torch.float16), frames,
-                                    h, w, C, _stream()), "pp_sc_fold_f16")
-    _count(1)
+    _launch("pp_sc_fold_f16", _p(cols, torch.float16), cols.stride(0), _pd(bmap), _pd(out, torch.float16), frames, h, w, C)
     return out
 
 
@@ -655,12 +584,10 @@ def pool_depthwise(x_pm, w_taps, bias, kh, kw):
     """depthwise conv, kernel = stride = (kh,kw): x_pm [n,H,W,C] -> [n,H//kh,W//kw,C]; w_taps [kh*kw, C].  fp16 x_pm (the
     half-operand LayerNorm output): fp16 out, weights / bias / sums fp32."""
     n, H, W, C = x_pm.shape
-    xp, ld = _pm(x_pm, x_pm.dtype)
-    out = torch.empty(n, (H - kh) // kh + 1, (W - kw) // kw + 1, C, device=x_pm.device, dtype=x_pm.dtype)
-    fn, name = ((_lib.lib().pp_pool_depthwise_f16, "pp_pool_depthwise_f16") if x_pm.dtype == torch.float16 else
-                (_lib.lib().pp_pool_depthwise, "pp_pool_depthwise"))
-    check(fn(xp, ld, _p(_dense(w_taps)), _p(bias), _p(out, x_pm.dtype), n, H, W, C, kh, kw, _stream()), name)
-    _count(1)
+    sym, dt = _twin("pp_pool_depthwise", x_pm)
+    xp, ld = _pm(x_pm, dt)
+    out = torch.empty(n, (H - kh) // kh + 1, (W - kw) // kw + 1, C, device=x_pm.device, dtype=dt)
+    _launch(sym, xp, ld, _pd(w_taps), _p(bias), _p(out, dt), n, H, W, C, kh, kw)
     return out
 
 
@@ -670,17 +597,12 @@ def add_layernorm(x, delta, gamma, beta, eps=1e-5, y_dtype=torch.float32):
     C = x.shape[-1]
     y = torch.empty_like(x, dtype=y_dtype)
     xo = torch.empty_like(x) if delta is not None else None
-    if torch.float16 in (y_dtype, delta.dtype if delta is not None else None):
-        dt = delta.dtype if delta is not None else torch.float32
-        check(_lib.lib().pp_add_layernorm_f16(_p(_dense(x)), _p(_dense(delta), dt) if delta is not None else None,
-                                              int(dt == torch.float16), _p(gamma), _p(beta), _p(xo), _p(y, y_dtype),
-                                              int(y_dtype == torch.float16), x.numel() // C, C, float(eps), _stream()),
-              "pp_add_layernorm_f16")
-        _count(1)
-        return (xo if delta is not None else x), y
-    check(_lib.lib().pp_add_layernorm(_p(_dense(x)), _p(_dense(delta)) if delta is not None else None, _p(gamma), _p(beta),
-                                      _p(xo), _p(y), x.numel() // C, C, float(eps), _stream()), "pp_add_layernorm")
-    _count(1)
+    dt = delta.dtype if delta is not None else torch.float32
+    if torch.float16 in (y_dtype, dt):
+        _launch("pp_add_layernorm_f16", _pd(x), _pd(delta, dt), int(dt == torch.float16), _p(gamma), _p(beta), _p(xo),
+                _p(y, y_dtype), int(y_dtype == torch.float16), x.numel() // C, C, float(eps))
+    else:
+        _launch("pp_add_layernorm", _pd(x), _pd(delta), _p(gamma), _p(beta), _p(xo), _p(y), x.numel() // C, C, float(eps))
     return (xo if delta is not None else x), y
 
 
@@ -688,13 +610,10 @@ def instance_norm(x_pm, relu=False, res=None, post_relu=False, eps=1e-5, out=Non
     """InstanceNorm2d(affine=False) on a dense pixel-major map [n,h,w,C] (+ ReLU, + residual add, + final ReLU)."""
     n, h, w, C = x_pm.shape
     out = torch.empty_like(x_pm) if out is None else out
-    lib = _lib.lib()
-    nbytes = lib.pp_instance_norm_workspace_bytes(n, h * w, C)
+    nbytes = _lib.lib().pp_instance_norm_workspace_bytes(n, h * w, C)
     ws = torch.empty(max(nbytes // 4, 4), device=x_pm.device, dtype=torch.float32)
-    check(lib.pp_instance_norm(_p(_dense(x_pm)), _p(_dense(res)) if res is not None else None, _p(_dense(out)), n, h * w, C,
-                               float(eps), int(bool(relu)), int(bool(post_relu)), _p(ws), ws.numel() * 4, _stream()),
-          "pp_instance_norm")
-    _count(2)
+    _launch("pp_instance_norm", _pd(x_pm), _pd(res), _pd(out), n, h * w, C, float(eps), int(bool(relu)), int(bool(post_relu)),
+            _p(ws), ws.numel() * 4, launches=2)
     return out
 
 
@@ -703,12 +622,8 @@ def upsample2x(x_pm):
     blended in fp32."""
     n, h, w, C = x_pm.shape
     out = torch.empty(n, 2 * h, 2 * w, C, device=x_pm.device, dtype=x_pm.dtype)
-    if x_pm.dtype == torch.float16:
-        check(_lib.lib().pp_upsample2x_bilinear_f16(_p(_dense(x_pm), torch.float16), _p(out, torch.float16), n, h, w, C, _stream()),
-              "pp_upsample2x_bilinear_f16")
-    else:
-        check(_lib.lib().pp_upsample2x_bilinear(_p(_dense(x_pm)), _p(out), n, h, w, C, _stream()), "pp_upsample2x_bilinear")
-    _count(1)
+    sym, dt = _twin("pp_upsample2x_bilinear", x_pm)
+    _launch(sym, _pd(x_pm, dt), _p(out, dt), n, h, w, C)
     return out
 
 
@@ -716,9 +631,7 @@ def mask_dilate(masks_u8, iterations):
     """uint8 [T,H,W] (non-zero = hole) -> float {0,1} [T,1,H,W], dilated `iterations` times with the 3x3 cross."""
     T, H, W = masks_u8.shape
     out = torch.empty(T, 1, H, W, device=masks_u8.device, dtype=torch.float32)
-    check(_lib.lib().pp_mask_dilate(_p(_dense(masks_u8), torch.uint8), _p(out), T, H, W, int(iterations), _stream()),
-          "pp_mask_dilate")
-    _count(1)
+    _launch("pp_mask_dilate", _pd(masks_u8, torch.uint8), _p(out), T, H, W, int(iterations))
     return out
 
 
@@ -726,8 +639,7 @@ def u8_to_frames(frames_u8):
     """uint8 [T,H,W,3] -> float planar [T,3,H,W] in [-1,1]."""
     T, H, W, _ = frames_u8.shape
     out = torch.empty(T, 3, H, W, device=frames_u8.device, dtype=torch.float32)
-    check(_lib.lib().pp_u8_to_frames(_p(_dense(frames_u8), torch.uint8), _p(out), T, H, W, _stream()), "pp_u8_to_frames")
-    _count(1)
+    _launch("pp_u8_to_frames", _pd(frames_u8, torch.uint8), _p(out), T, H, W)
     return out
 
 
@@ -742,23 +654,13 @@ def u8_to_frames_resized(frames_u8, size):
     if w < 1 or h < 1 or H0 < 1 or W0 < 1:
         raise ValueError(f"u8_to_frames_resized: cannot resize {H0}x{W0} frames to size {tuple(size)}")
     out = torch.empty(T, 3, h, w, device=frames_u8.device, dtype=torch.float32)
-    check(_lib.lib().pp_u8_to_frames_resized(_p(_dense(frames_u8), torch.uint8), _p(out), T, H0, W0, h, w, _stream()),
-          "pp_u8_to_frames_resized")
-    _count(1)
+    _launch("pp_u8_to_frames_resized", _pd(frames_u8, torch.uint8), _p(out), T, H0, W0, h, w)
     return out
 
 
 def composite_blend(pred, masks, ori_u8, comp_u8, frame_ids, first_flags):
     """pred [n,3,H,W]; masks [T,1,H,W]; ori/comp uint8 [T,H,W,3] (comp updated in place)."""
-    n, _, H, W = pred.shape
-    ids = PPWindowIds()
-    ids.n = n
-    for i, (f, fl) in enumerate(zip(frame_ids, first_flags)):
-        ids.frame[i], ids.first[i] = int(f), int(fl)
-    check(_lib.lib().pp_composite_blend_u8(_p(_dense(pred)), _p(_dense(masks)), _p(_dense(ori_u8), torch.uint8),
-                                           _p(_dense(comp_u8), torch.uint8), ctypes.byref(ids), H, W, _stream()),
-          "pp_composite_blend_u8")
-    _count(1)
+    _composite_blend("pp_composite_blend_u8", torch.uint8, pred, masks, ori_u8, comp_u8, frame_ids, first_flags)
 
 
 def composite_blend_f32(pred, masks, ori_u8, comp_f32, frame_ids, first_flags):
@@ -766,15 +668,16 @@ def composite_blend_f32(pred, masks, ori_u8, comp_f32, frame_ids, first_flags):
     clip [T,H,W,3] (updated in place) and a later visit's 1/2-1/2 blend is not truncated."""
     if comp_f32.dtype != torch.float32:
         raise RuntimeError(f"composite_blend_f32: comp must be float32, got {comp_f32.dtype}")
+    _composite_blend("pp_composite_blend_f32", torch.float32, pred, masks, ori_u8, comp_f32, frame_ids, first_flags)
+
+
+def _composite_blend(sym, comp_dtype, pred, masks, ori_u8, comp, frame_ids, first_flags):
     n, _, H, W = pred.shape
     ids = PPWindowIds()
     ids.n = n
     for i, (f, fl) in enumerate(zip(frame_ids, first_flags)):
         ids.frame[i], ids.first[i] = int(f), int(fl)
-    check(_lib.lib().pp_composite_blend_f32(_p(_dense(pred)), _p(_dense(masks)), _p(_dense(ori_u8), torch.uint8),
-                                            _p(_dense(comp_f32)), ctypes.byref(ids), H, W, _stream()),
-          "pp_composite_blend_f32")
-    _count(1)
+    _launch(sym, _pd(pred), _pd(masks), _pd(ori_u8, torch.uint8), _pd(comp, comp_dtype), ctypes.byref(ids), H, W)
 
 
 def extrapolate_u8(frames_u8, geometry):
@@ -785,14 +688,12 @@ def extrapolate_u8(frames_u8, geometry):
     if frames_u8.dim() != 4 or frames_u8.shape[-1] != 3:
         raise RuntimeError("extrapolate_u8: expected uint8 frames [T,h,w,3]")
     T, h, w, _ = frames_u8.shape
-    src = _p(_dense(frames_u8), torch.uint8)
+    src = _pd(frames_u8, torch.uint8)
     dev = frames_u8.device
     canvas = torch.empty(T, H, W, 3, dtype=torch.uint8, device=dev)
     fm = torch.empty(T, 1, H, W, dtype=torch.float32, device=dev)
     md = torch.empty_like(fm)
-    check(_lib.lib().pp_extrapolate_u8(src, _p(canvas, torch.uint8), _p(fm), _p(md), T, h, w, H, W, top, left, rim_h, rim_w,
-                                       _stream()), "pp_extrapolate_u8")
-    _count(1)
+    _launch("pp_extrapolate_u8", src, _p(canvas, torch.uint8), _p(fm), _p(md), T, h, w, H, W, top, left, rim_h, rim_w)
     return canvas, fm, md
 
 
@@ -805,9 +706,7 @@ def mask_overlay_u8(frames_u8, masks):
     if masks.numel() != T * H * W or tuple(masks.shape[-2:]) != (H, W):
         raise RuntimeError(f"mask_overlay_u8: masks {tuple(masks.shape)} do not match frames {tuple(frames_u8.shape)}")
     out = torch.empty_like(frames_u8)
-    check(_lib.lib().pp_mask_overlay_u8(_p(_dense(frames_u8), torch.uint8), _p(_dense(masks)), _p(out, torch.uint8), T, H, W,
-                                        _stream()), "pp_mask_overlay_u8")
-    _count(1)
+    _launch("pp_mask_overlay_u8", _pd(frames_u8, torch.uint8), _pd(masks), _p(out, torch.uint8), T, H, W)
     return out
 
 
@@ -835,11 +734,9 @@ def flow_to_image_u8(flow, normalize="frame", clip_flow=None, bgr=False):
     maxima = torch.empty(N if per_frame else 1, dtype=torch.float32, device=f.device)
     out = torch.empty(N, H, W, 3, dtype=torch.uint8, device=f.device)
     has_clip, clip = int(clip_flow is not None), ctypes.c_float(0.0 if clip_flow is None else float(clip_flow))
-    L = _lib.lib()
-    check(L.pp_flow_maxrad(_p(f), _p(maxima), N, H, W, per_frame, has_clip, clip, _stream()), "pp_flow_maxrad")
-    check(L.pp_flow_to_image_u8(_p(f), _p(maxima), _p(out, torch.uint8), N, H, W, FLOWVIZ_NORMALIZE[normalize], has_clip,
-                                clip, int(bool(bgr)), _stream()), "pp_flow_to_image_u8")
-    _count(2)
+    _launch("pp_flow_maxrad", _p(f), _p(maxima), N, H, W, per_frame, has_clip, clip)
+    _launch("pp_flow_to_image_u8", _p(f), _p(maxima), _p(out, torch.uint8), N, H, W, FLOWVIZ_NORMALIZE[normalize], has_clip, clip,
+            int(bool(bgr)))
     return out[0] if single else out
 
 
@@ -873,8 +770,7 @@ def flow_occlusion(fw, bw):
     f, b = _ewarp_dev("flow_occlusion", f, b)
     N, _, H, W = f.shape
     occ = torch.empty(N, H, W, dtype=torch.uint8, device=f.device)
-    check(_lib.lib().pp_flow_occlusion(_p(f), _p(b), _p(occ, torch.uint8), N, H, W, _stream()), "pp_flow_occlusion")
-    _count(1)
+    _launch("pp_flow_occlusion", _p(f), _p(b), _p(occ, torch.uint8), N, H, W)
     return occ
 
 
@@ -904,12 +800,10 @@ def warp_error_sums(frames_u8, fw, occ=None, bw=None):
     else:
         raise ValueError("warp_error: needs the occlusion map `occ` or the backward flows `bw`")
     fr, f, b, o = _ewarp_dev("warp_error", frames_u8, f, b, occ)
-    L = _lib.lib()
-    ws = torch.empty(L.pp_warp_error_workspace_bytes(T, H, W), dtype=torch.uint8, device=f.device)
+    ws = torch.empty(_lib.lib().pp_warp_error_workspace_bytes(T, H, W), dtype=torch.uint8, device=f.device)
     out = torch.empty(T - 1, 2, dtype=torch.float64, device=f.device)
-    check(L.pp_warp_error(_p(fr, torch.uint8), _p(f), _p(b), _p(o, torch.uint8), _p(out, torch.float64), T, H, W,
-                          _p(ws, torch.uint8), ws.numel(), _stream()), "pp_warp_error")
-    _count(2)
+    _launch("pp_warp_error", _p(fr, torch.uint8), _p(f), _p(b), _p(o, torch.uint8), _p(out, torch.float64), T, H, W,
+            _p(ws, torch.uint8), ws.numel(), launches=2)
     return out
 
 
@@ -948,11 +842,10 @@ def i3d_input(video):
         if video.shape[1] != 3:
             raise RuntimeError("i3d_input: float video must be [B,3,T,H,W]")
         B, _, T, H, W = video.shape
-    src = _p(_dense(video), video.dtype if u8 else torch.float32)
+    src = _pd(video, video.dtype if u8 else torch.float32)
     out = torch.empty(B, T + same_pad(7, 2, T), H + same_pad(7, 2, H), W + same_pad(7, 2, W), 4, device=video.device,
                       dtype=torch.float32)
-    check(_lib.lib().pp_i3d_input(src, int(u8), _p(out), B, T, H, W, _stream()), "pp_i3d_input")
-    _count(1)
+    _launch("pp_i3d_input", src, int(u8), _p(out), B, T, H, W)
     return out
 
 
@@ -968,8 +861,7 @@ def maxpool3d_same(x, kernel, stride, out=None):
         raise RuntimeError(f"maxpool3d_same: out {tuple(out.shape)} != {shape}")
     xp, ldx = _pm(x)
     op, ldo = _pm(out)
-    check(_lib.lib().pp_maxpool3d_same(xp, ldx, op, ldo, B, T, H, W, C, kt, kh, kw, st, sh, sw, _stream()), "pp_maxpool3d_same")
-    _count(1)
+    _launch("pp_maxpool3d_same", xp, ldx, op, ldo, B, T, H, W, C, kt, kh, kw, st, sh, sw)
     return out
 
 
@@ -979,8 +871,7 @@ def mean_thw(x):
     B, C = x.shape[0], x.shape[-1]
     xp, ld = _pm(x)
     out = torch.empty(B, C, device=x.device, dtype=torch.float32)
-    check(_lib.lib().pp_mean_thw(xp, ld, _p(out), B, x[0, ..., 0].numel(), C, _stream()), "pp_mean_thw")
-    _count(1)
+    _launch("pp_mean_thw", xp, ld, _p(out), B, x[0, ..., 0].numel(), C)
     return out
 
 
@@ -1030,13 +921,11 @@ def resize_frames_u8(frames_u8, size):
     bx, kx = resample_tables("bicubic", W, Wo, dev)
     by, ky = resample_tables("bicubic", H, Ho, dev)
     out = torch.empty(T, Ho, Wo, 3, dtype=torch.uint8, device=dev)
-    L = _lib.lib()
-    nws = L.pp_resize_u8_bicubic_workspace_bytes(T, H, Wo)
+    nws = _lib.lib().pp_resize_u8_bicubic_workspace_bytes(T, H, Wo)
     ws = torch.empty(max(nws, 16), dtype=torch.uint8, device=dev)
-    check(L.pp_resize_u8_bicubic(_p(_dense(frames_u8), torch.uint8), _p(out, torch.uint8), T, H, W, Ho, Wo, _p(bx, torch.int32), _p(kx, torch.int32),
-                                 kx.shape[1], _p(by, torch.int32), _p(ky, torch.int32), ky.shape[1], _p(ws, torch.uint8), ws.numel(), _stream()),
-          "pp_resize_u8_bicubic")
-    _count(2)
+    _launch("pp_resize_u8_bicubic", _pd(frames_u8, torch.uint8), _p(out, torch.uint8), T, H, W, Ho, Wo, _p(bx, torch.int32),
+            _p(kx, torch.int32), kx.shape[1], _p(by, torch.int32), _p(ky, torch.int32), ky.shape[1], _p(ws, torch.uint8),
+            ws.numel(), launches=2)
     return out
 
 
@@ -1047,9 +936,8 @@ def resize_masks_u8(masks_u8, size):
     dev = masks_u8.device
     (ix,), (iy,) = resample_tables("nearest", W, Wo, dev), resample_tables("nearest", H, Ho, dev)
     out = torch.empty(T, Ho, Wo, dtype=torch.uint8, device=dev)
-    check(_lib.lib().pp_resize_u8_nearest(_p(_dense(masks_u8), torch.uint8), _p(out, torch.uint8), T, H, W, Ho, Wo, 1, _p(ix, torch.int32),
-                                          _p(iy, torch.int32), _stream()), "pp_resize_u8_nearest")
-    _count(1)
+    _launch("pp_resize_u8_nearest", _pd(masks_u8, torch.uint8), _p(out, torch.uint8), T, H, W, Ho, Wo, 1, _p(ix, torch.int32),
+            _p(iy, torch.int32))
     return out
 
 
@@ -1061,9 +949,8 @@ def resize_output_u8(frames_u8, size):
     xo, xa = resample_tables("linear_cv", W, Wo, dev, True)
     yo, ya = resample_tables("linear_cv", H, Ho, dev, False)
     out = torch.empty(T, Ho, Wo, 3, dtype=torch.uint8, device=dev)
-    check(_lib.lib().pp_resize_u8_bilinear_cv(_p(_dense(frames_u8), torch.uint8), _p(out, torch.uint8), T, H, W, Ho, Wo, _p(xo, torch.int32),
-                                              _p(xa, torch.int16), _p(yo, torch.int32), _p(ya, torch.int16), _stream()), "pp_resize_u8_bilinear_cv")
-    _count(1)
+    _launch("pp_resize_u8_bilinear_cv", _pd(frames_u8, torch.uint8), _p(out, torch.uint8), T, H, W, Ho, Wo, _p(xo, torch.int32),
+            _p(xa, torch.int16), _p(yo, torch.int32), _p(ya, torch.int16))
     return out
 
 
@@ -1081,9 +968,8 @@ def resize_flow(flows, size):
     xo, xa = resample_tables("linear_f32", W, Wo, dev, True)
     yo, ya = resample_tables("linear_f32", H, Ho, dev, False)
     out = torch.empty(N, 2, Ho, Wo, dtype=torch.float32, device=dev)
-    check(_lib.lib().pp_resize_flow_linear_cv(_p(_dense(flows)), _p(out), N, H, W, Ho, Wo, _p(xo, torch.int32), _p(xa),
-                                              _p(yo, torch.int32), _p(ya), _stream()), "pp_resize_flow_linear_cv")
-    _count(1)
+    _launch("pp_resize_flow_linear_cv", _pd(flows), _p(out), N, H, W, Ho, Wo, _p(xo, torch.int32), _p(xa), _p(yo, torch.int32),
+            _p(ya))
     return out
 
 
@@ -1115,11 +1001,8 @@ def cutie_topk_readout(mem_key, mem_shrink, mem_value, n_frames, fifo_head, fifo
     if want_selection:
         sel_idx = torch.empty(HW, top_k, device=qk.device, dtype=torch.int32)
         sel_w = torch.empty(HW, top_k, device=qk.device, dtype=torch.float32)
-    check(_lib.lib().pp_cutie_topk_readout(_p(_dense(mem_key)), _p(_dense(mem_shrink)), _p(mem_value), mem_value.stride(0),
-                                           n_frames, fifo_head, fifo_cap, _p(_dense(qk)), _p(_dense(qe)), HW, nobj, top_k,
-                                           _p(_dense(out)), _p(sel_idx, torch.int32), _p(sel_w), _stream()),
-          "pp_cutie_topk_readout")
-    _count(1)
+    _launch("pp_cutie_topk_readout", _pd(mem_key), _pd(mem_shrink), _p(mem_value), mem_value.stride(0), n_frames, fifo_head,
+            fifo_cap, _pd(qk), _pd(qe), HW, nobj, top_k, _pd(out), _p(sel_idx, torch.int32), _p(sel_w))
     return (out, sel_idx, sel_w) if want_selection else out
 
 
@@ -1131,8 +1014,7 @@ def cutie_frame_in(frame_u8, out=None):
     Hp, Wp = -(-H // 16) * 16, -(-W // 16) * 16
     if out is None:
         out = torch.empty(1, 3, Hp, Wp, device=frame_u8.device, dtype=torch.float32)
-    check(_lib.lib().pp_cutie_frame_in(_p(_dense(frame_u8), torch.uint8), _p(_dense(out)), H, W, _stream()), "pp_cutie_frame_in")
-    _count(1)
+    _launch("pp_cutie_frame_in", _pd(frame_u8, torch.uint8), _pd(out), H, W)
     return out
 
 
@@ -1143,9 +1025,7 @@ def cutie_labels(prob, lut, H, W, out=None):
         raise RuntimeError(f"cutie_labels: prob {tuple(prob.shape)} / lut {tuple(lut.shape)} do not fit {H}x{W}")
     if out is None:
         out = torch.empty(H, W, device=prob.device, dtype=torch.uint8)
-    check(_lib.lib().pp_cutie_labels(_p(_dense(prob)), K, _p(_dense(lut), torch.uint8), _p(_dense(out), torch.uint8), H, W,
-                                     _stream()), "pp_cutie_labels")
-    _count(1)
+    _launch("pp_cutie_labels", _pd(prob), K, _pd(lut, torch.uint8), _pd(out, torch.uint8), H, W)
     return out
 
 
@@ -1211,10 +1091,8 @@ def mask_paint_u8(frames_u8, labels_u8, palette=None, mask_alpha=0.7, out=None):
         out = torch.empty_like(frames_u8)
     elif not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.shape != frames_u8.shape or out.device != frames_u8.device:
         raise ValueError("mask_paint_u8: out must be a uint8 tensor shaped and placed like frames_u8")
-    L = _lib.lib()
-    ws = torch.empty(L.pp_mask_paint_workspace_bytes(T, H, W), dtype=torch.uint8, device=frames_u8.device)
-    check(L.pp_mask_paint_u8(_p(_dense(frames_u8), torch.uint8), _p(_dense(labels_u8), torch.uint8), _p(pal, torch.uint8), N,
-                             (ctypes.c_double * 2)(alpha, 1.0 - alpha), _p(_dense(out), torch.uint8), T, H, W,
-                             _p(ws, torch.uint8), ws.numel(), _stream()), "pp_mask_paint_u8")
-    _count(3)
+    ws = torch.empty(_lib.lib().pp_mask_paint_workspace_bytes(T, H, W), dtype=torch.uint8, device=frames_u8.device)
+    _launch("pp_mask_paint_u8", _pd(frames_u8, torch.uint8), _pd(labels_u8, torch.uint8), _p(pal, torch.uint8), N,
+            (ctypes.c_double * 2)(alpha, 1.0 - alpha), _pd(out, torch.uint8), T, H, W, _p(ws, torch.uint8), ws.numel(),
+            launches=3)
     return out
